@@ -1172,7 +1172,6 @@ int gx_set_graph_batch_csr(gx_handle* h, int32_t G, int32_t max_nodes, const int
 int gx_plan_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int64_t* edge_off, int64_t* total_edges) {
   if (!h || !graph_ids) { gx_set_error("gx_plan_graphs: NULL argument"); return GX_ERR_INVALID; }
   if (!h->has_batch || !h->has_model) { gx_set_error("gx_plan_graphs: call gx_set_model and gx_set_graph_batch_csr first"); return GX_ERR_INVALID; }
-  if (h->m.variant) { gx_set_error("gx_plan_graphs: graph mode builds the default model only (3 layers, no --bn)"); return GX_ERR_UNSUPPORTED; }
   if (h->gb.d != h->m.d) { gx_set_error("gx_plan_graphs: feat_dim %d != model input_dim %d", h->gb.d, h->m.d); return GX_ERR_INVALID; }
   if (count <= 0) { gx_set_error("gx_plan_graphs: count <= 0"); return GX_ERR_INVALID; }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
@@ -1194,10 +1193,12 @@ int gx_plan_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int64_
     T.e_d = rp[nf] - rp[0]; T.e1 = T.e_d; T.npairs = T.e_d / 2; T.npairs_in = T.npairs;
     T.gt_label = h->gb_h_label[g]; T.n_norm = nf; T.flags = na < nf ? 1 : 0;
     T.node_off = tn; T.rp_off = tn + t; T.edge_off = te; T.pair_off = tp;
-    if (na >= 65535 || T.e_d >= 65535) { gx_set_error("gx_plan_graphs: graph %d too large for the shared-memory kernel", g); return GX_ERR_UNSUPPORTED; }
-    const GxLayoutG L = gx_make_layout_graph(na, T.e_d, T.npairs, h->m.d, h->m.hid, h->m.emb, h->m.C, nwarps);
-    T.smem_bytes = L.total_words * 4;
-    if (T.smem_bytes > 226 * 1024) { gx_set_error("gx_plan_graphs: graph %d needs %d bytes of shared memory", g, T.smem_bytes); return GX_ERR_UNSUPPORTED; }
+    if (!h->m.variant) {   // the tuned kernel (explain_graph.cu) keeps a graph in shared memory with 16-bit indices
+      if (na >= 65535 || T.e_d >= 65535) { gx_set_error("gx_plan_graphs: graph %d too large for the shared-memory kernel", g); return GX_ERR_UNSUPPORTED; }
+      const GxLayoutG L = gx_make_layout_graph(na, T.e_d, T.npairs, h->m.d, h->m.hid, h->m.emb, h->m.C, nwarps);
+      T.smem_bytes = L.total_words * 4;
+      if (T.smem_bytes > 226 * 1024) { gx_set_error("gx_plan_graphs: graph %d needs %d bytes of shared memory", g, T.smem_bytes); return GX_ERR_UNSUPPORTED; }
+    }   // model variants: explain_graph_var.cu keeps a graph in a global slab (smem_bytes 0: one launch class), bounded by max_nodes <= 4096
     max_smem = std::max(max_smem, T.smem_bytes); max_np = std::max(max_np, T.npairs);
     tn += na; te += T.e_d; tp += T.npairs;
   }
@@ -1255,6 +1256,12 @@ static int explain_graphs_impl(gx_handle* h, const gx_hparams* hp, gx_memspace s
   if (hp->mask_act != 0) { gx_set_error("gx_explain_graphs: mask_act != sigmoid is not built (the reference's ReLU variant returns NaN masks)"); return GX_ERR_UNSUPPORTED; }
   if (hp->num_epochs < 1) { gx_set_error("gx_explain_graphs: num_epochs < 1"); return GX_ERR_INVALID; }
   if (hp->init != GX_INIT_M0 && hp->init != GX_INIT_PHILOX && hp->init != GX_INIT_STATE) { gx_set_error("gx_explain_graphs: unknown init %d", hp->init); return GX_ERR_INVALID; }
+  { const int orc = check_optimiser("gx_explain_graphs", hp); if (orc != GX_OK) return orc; }
+  const bool var = h->m.variant || hp->opt != GX_OPT_ADAM;   // the whole batch through explain_graph_var.cu
+  if (var && (hp->init == GX_INIT_STATE || (io && (io->trace || io->trace_pred || io->adam_m_out || io->adam_v_out || io->mask_param_out || io->feat_state_out)))) {
+    gx_set_error("gx_explain_graphs: model variants (num_layers != 3 / --bn / widths > 32) and optimisers other than Adam build the mask optimisation only (no trace or optimiser state)");
+    return GX_ERR_UNSUPPORTED;
+  }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
   const int count = h->g_count;
   const int64_t te = h->g_total_e;
@@ -1262,15 +1269,47 @@ static int explain_graphs_impl(gx_handle* h, const gx_hparams* hp, gx_memspace s
   int rc = io_prepare(h, "gx_explain_graphs", hp, 0, space, io, count, te, h->m.d, h->m.C, &D);
   if (rc != GX_OK) return rc;
   D.x.tr_outer = nullptr;   // graph mode has no outer pairs
-  rc = check_optimiser("gx_explain_graphs", hp);
-  if (rc != GX_OK) return rc;
-  if (hp->opt != GX_OPT_ADAM) { gx_set_error("gx_explain_graphs: graph mode builds Adam only (the schedulers work)"); return GX_ERR_UNSUPPORTED; }
   GxHparamsDev hd;
   fill_hparams(h, hp, 0, D.x.trace != nullptr, &hd);
   hd.c_lap = 0.f;           // lap_loss = 0 in graph mode (explain.py:787-788)
   rc = upload_adam_table(h, hp, hd.iters, hp->start_step);
   if (rc != GX_OK) return rc;
   hd.adam_tab = h->d_adam.as<float2>();
+  if (var) {
+    // one persistent launch over the whole batch, largest graphs first (d_order); per CTA a global slab for one graph and 8 floats per edge
+    if (gx_graph_var_smem_bytes(h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C) > gx_explain_max_smem()) { gx_set_error("gx_explain_graphs: model does not fit the variant kernel"); return GX_ERR_UNSUPPORTED; }
+    const int vw = gx_var_row_stride(h->m.hid, h->m.emb);
+    int64_t words = 4; int maxnp = 0;
+    for (const GxTask& T : h->tasks) {
+      words = std::max<int64_t>(words, gx_make_graph_var_layout(T.n, T.e_d, h->m.d, h->m.L, vw).total_words);
+      maxnp = std::max(maxnp, T.npairs);
+    }
+    const int64_t pstride = ((int64_t)maxnp * 8 + 3) / 4 * 4 + 4;
+    const int per_sm = gx_graph_var_ctas_per_sm(h->m);
+    if (per_sm < 1) { gx_set_error("gx_explain_graphs: the variant kernel cannot be resident (%d bytes of shared memory)", gx_graph_var_smem_bytes(h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C)); return GX_ERR_UNSUPPORTED; }
+    int grid = std::min(count, h->num_sms * per_sm);
+    const int64_t per_cta = (words + pstride) * 4;
+    size_t free_b = 0, total_b = 0;
+    GX_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+    const int64_t budget = (int64_t)(free_b + h->d_gws.cap + h->d_pws.cap) * 8 / 10;
+    if (per_cta > budget) { gx_set_error("gx_explain_graphs: a graph needs %lld MB of device workspace, %lld MB are free", (long long)(per_cta >> 20), (long long)(budget >> 20)); return GX_ERR_CUDA; }
+    grid = (int)std::max<int64_t>(1, std::min<int64_t>(grid, budget / per_cta));
+    GX_CUDA_CHECK(h->d_gws.reserve((size_t)grid * words * 4));
+    GX_CUDA_CHECK(h->d_pws.reserve((size_t)grid * pstride * 4));
+    GX_CUDA_CHECK(cudaMemsetAsync(h->d_counters.p, 0, kNumClasses * 4, h->stream));
+    GX_CUDA_CHECK(cudaEventRecord(h->ev_t0, h->stream));
+    GxExplainLaunch cfg;
+    cfg.order = h->d_order.as<int32_t>(); cfg.ntasks = count; cfg.counter = h->d_counters.as<int32_t>();
+    cfg.smem_bytes = 0; cfg.threads = 0; cfg.grid = grid;
+    cfg.gws = h->d_gws.as<float>(); cfg.gws_stride_words = words;
+    cfg.pws = h->d_pws.as<float>(); cfg.pws_stride_words = pstride;
+    cfg.dbg = nullptr; cfg.x = D.x;
+    GX_CUDA_CHECK(gx_launch_explain_graph_var(cfg, h->gb, h->m, hd, h->plan, D.m0, D.out, D.feat, h->stream));
+    h->launches += 1;
+    GX_CUDA_CHECK(cudaEventRecord(h->ev_t1, h->stream));
+    h->timed = true;
+    return io_finish(h, hp, space, io, count, te, h->m.d, h->m.C, D);
+  }
   // one persistent launch per footprint class, on its own stream (the classes overlap like the node-mode classes)
   int grids[6]; int64_t pstride[6], poff[7] = {};
   for (int c = 0; c < 6; ++c) {

@@ -8,40 +8,9 @@
 // kernel is written for clarity, not speed: one persistent CTA per task, state in a per-CTA global slab (L2 resident for the
 // reference's graph sizes), one warp per row with lane = feature, one thread per undirected edge in the edge phase.
 // Phases per epoch (one __syncthreads each): F1 .. FL | S | BL .. B1 | P.  The default model (3 layers, no bn) never comes here.
-#include "explain_common.cuh"
+#include "explain_var_common.cuh"
 
 namespace {
-
-constexpr int kVarThreads = 256;
-constexpr int kVarWeightWords = 36 * 1024;   // conv weights are staged in shared memory up to this many floats (144 KB), read through L2 beyond
-
-// KW = 32-lane chunks of a hidden-width row (lane = feature, chunk k holds features 32k + lane): 1 for widths <= 32, 2 <= 64, 4 <= 128
-__host__ __device__ inline int var_kw(int hid, int emb) { const int w = hid > emb ? hid : emb; return w <= 32 ? 1 : (w <= 64 ? 2 : 4); }
-
-struct VarSmem { int W[GX_MAX_LAYERS], b[GX_MAX_LAYERS], Wp, sF, F, mF, vF, zs, zlen, gFp, emb, dEmb, logit, w_in_smem, total; };
-__host__ __device__ inline VarSmem var_smem(int d, int L, int hid, int emb, int C, int nwarps) {
-  VarSmem S;
-  const int dp = gx_round_up(d, 4);
-  int o = 0;
-  auto take = [&](int words) { int r = o; o += gx_round_up(words, 4); return r; };
-  int wwords = 0;
-  for (int l = 0; l < L; ++l) wwords += (l == 0 ? d : hid) * (l == L - 1 ? emb : hid);
-  S.w_in_smem = wwords <= kVarWeightWords;
-  for (int l = 0; l < L; ++l) {
-    const int win = l == 0 ? d : hid, wout = l == L - 1 ? emb : hid;
-    S.W[l] = take(S.w_in_smem ? win * wout : 0);
-    S.b[l] = take(wout);
-  }
-  const int PD = hid * (L - 1) + emb;
-  S.Wp = take(C * (PD + 1) <= GX_WP_SMEM_MAX ? C * (PD + 1) : 0);
-  S.sF = take(dp); S.F = take(dp); S.mF = take(dp); S.vF = take(dp);
-  S.zlen = dp > 32 * var_kw(hid, emb) ? dp : 32 * var_kw(hid, emb);   // per-warp scratch row: a feature row or a hidden row
-  S.zs = take(nwarps * S.zlen);
-  S.gFp = take(nwarps * dp);
-  S.emb = take(PD); S.dEmb = take(PD); S.logit = take(C < 32 ? 32 : C);
-  S.total = o;
-  return S;
-}
 
 template <bool kBn, int KW>
 __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainArgs A) {
@@ -68,17 +37,7 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
   auto wout_of = [&](int l) { return l == L - 1 ? embw : hid; };
 
   const float* Wl[GX_MAX_LAYERS];   // conv weights: shared memory when they fit, else global (L2 resident)
-  for (int l = 0; l < L; ++l) {
-    const int cnt = win_of(l) * wout_of(l);
-    if (S.w_in_smem)
-      for (int idx = tid; idx < cnt; idx += NT) sm[S.W[l] + idx] = __ldg(m.W[l] + idx);
-    Wl[l] = S.w_in_smem ? sm + S.W[l] : m.W[l];
-    for (int idx = tid; idx < wout_of(l); idx += NT) sm[S.b[l] + idx] = __ldg(m.b[l] + idx);
-  }
-  if (wp_smem) {
-    for (int idx = tid; idx < C * PD; idx += NT) sm[S.Wp + idx] = __ldg(m.Wp + idx);
-    for (int idx = tid; idx < C; idx += NT) sm[S.Wp + C * PD + idx] = __ldg(m.bp + idx);
-  }
+  var_stage_model(m, S, sm, Wl, tid, NT);
   float* const slab = A.gws + (int64_t)blockIdx.x * A.gws_stride_words;
   float2* const MM0 = reinterpret_cast<float2*>(A.pws + (int64_t)blockIdx.x * A.pws_stride_words);
 
@@ -122,14 +81,8 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
       const float m0_std = sqrtf(2.0f / (float)n);  // gain('relu') * sqrt(2/(n+n)) (explain.py:647-651)
       for (int p = tid; p < np; p += NT) {
         const int oij = poij[p], oji = poji[p];
-        float Mi, Mj;
-        if (hp.init == GX_INIT_PHILOX) {
-          Mi = 1.0f + m0_std * philox_normal(hp.seed, (uint32_t)Tp->node, (uint32_t)oij);
-          Mj = 1.0f + m0_std * philox_normal(hp.seed, (uint32_t)Tp->node, (uint32_t)oji);
-        } else {
-          Mi = __ldg(A.m0 + edge_off + oij);
-          Mj = __ldg(A.m0 + edge_off + oji);
-        }
+        const float Mi = var_init_param(hp, A.m0, edge_off + oij, (uint32_t)Tp->node, (uint32_t)oij, m0_std);
+        const float Mj = var_init_param(hp, A.m0, edge_off + oji, (uint32_t)Tp->node, (uint32_t)oji, m0_std);
         MM[p] = make_float2(Mi, Mj);
         mm[p] = make_float2(0.f, 0.f);
         vv[p] = make_float2(0.f, 0.f);
@@ -153,62 +106,15 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
         const float* const Ws = Wl[l - 1]; const float* const bsm = sm + S.b[l - 1];
         for (int i = warp; i < R[l]; i += nwarps) {
           const int r0 = irp[i], r1 = irp[i + 1];
+          if (l == 1) var_gather_feat(r0, r1, icol, a, A.g.feat, lo2gid, d, sF, U + (int64_t)i * dp, zs, lane);
+          else var_gather_hidden<KW>(r0, r1, icol, a, Hh(l - 1), win, zs, lane);
+          __syncwarp();
           float y[KW];
-#pragma unroll
-          for (int k = 0; k < KW; ++k) y[k] = lane + 32 * k < wout ? bsm[lane + 32 * k] : 0.f;
-          if (l == 1) {
-            for (int f0 = 0; f0 < d; f0 += 32) {
-              const int f = f0 + lane;
-              float z = 0.f;
-              if (f < d)
-                for (int e = r0; e < r1; ++e) z = fmaf(a[e], __ldg(A.g.feat + (int64_t)lo2gid[icol[e]] * d + f), z);
-              if (f < d) { U[(int64_t)i * dp + f] = z; zs[f] = z * sF[f]; }   // x * sigmoid(feat_mask) (explain.py:707), linear in x
-            }
-          } else {
-            const float* const Hp = Hh(l - 1);
-#pragma unroll
-            for (int k = 0; k < KW; ++k) {
-              const int f = lane + 32 * k;
-              float z = 0.f;
-              if (f < win)
-                for (int e = r0; e < r1; ++e) z = fmaf(a[e], Hp[(int64_t)icol[e] * VW + f], z);
-              if (f < win) zs[f] = z;
-            }
-          }
+          var_dense<KW>(zs, win, Ws, wout, bsm, y, lane);
           __syncwarp();
-          for (int f = 0; f < win; ++f) {
-            const float zf = zs[f];
-#pragma unroll
-            for (int k = 0; k < KW; ++k)
-              if (lane + 32 * k < wout) y[k] = fmaf(zf, Ws[f * wout + lane + 32 * k], y[k]);
-          }
-          __syncwarp();
-          float ssl = 0.f;
-#pragma unroll
-          for (int k = 0; k < KW; ++k) ssl += lane + 32 * k < wout ? y[k] * y[k] : 0.f;
-          const float ss = warp_sum(ssl);
-          const float q = fmaxf(sqrtf(ss), 1e-12f);   // F.normalize(p=2, dim=2), eps 1e-12
-          float yh[KW], h[KW];
-#pragma unroll
-          for (int k = 0; k < KW; ++k) { yh[k] = lane + 32 * k < wout ? y[k] / q : 0.f; h[k] = yh[k]; }
-          if (l < L) {
-#pragma unroll
-            for (int k = 0; k < KW; ++k) h[k] = fmaxf(yh[k], 0.f);
-            if (kBn) {   // fresh BatchNorm1d(n) in train mode: per node, over the feature axis (models.py:222-228)
-              float sl = 0.f;
-#pragma unroll
-              for (int k = 0; k < KW; ++k) sl += lane + 32 * k < wout ? h[k] : 0.f;
-              const float mu = warp_sum(sl) / (float)wout;
-              float vl = 0.f;
-#pragma unroll
-              for (int k = 0; k < KW; ++k) { h[k] = lane + 32 * k < wout ? h[k] - mu : 0.f; vl += h[k] * h[k]; }
-              const float var = warp_sum(vl) / (float)wout;
-              const float is = 1.0f / sqrtf(var + 1e-5f);
-#pragma unroll
-              for (int k = 0; k < KW; ++k) h[k] *= is;
-              if (lane == 0) istd(l)[i] = is;
-            }
-          }
+          float yh[KW], h[KW], is = 1.f;
+          const float q = var_activate<kBn, KW>(y, wout, l < L, yh, h, &is, lane);
+          if (kBn && l < L && lane == 0) istd(l)[i] = is;
 #pragma unroll
           for (int k = 0; k < KW; ++k) {
             Yh(l)[(int64_t)i * VW + lane + 32 * k] = yh[k];
@@ -223,27 +129,7 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
         for (int l = 1; l <= L; ++l)
           for (int c = lane; c < wout_of(l - 1); c += 32) emb[hid * (l - 1) + c] = Hh(l)[c];
         __syncwarp();
-        for (int c = 0; c < C; ++c) {
-          float t = 0.f;
-          for (int k = lane; k < PD; k += 32) t = fmaf(emb[k], Wpp[c * PD + k], t);
-          t = warp_sum(t);
-          if (lane == 0) logit[c] = t + bpp[c];
-        }
-        __syncwarp();
-        float mx = -INFINITY;
-        for (int c = lane; c < C; c += 32) mx = fmaxf(mx, logit[c]);
-        mx = warp_max(mx);
-        float se = 0.f;
-        for (int c = lane; c < C; c += 32) se += expf(logit[c] - mx);
-        se = warp_sum(se);
-        __syncwarp();
-        for (int c = lane; c < C; c += 32) logit[c] = expf(logit[c] - mx) / se - (c == gt ? 1.f : 0.f);  // p - onehot(gt) (explain.py:750-753)
-        __syncwarp();
-        for (int k = lane; k < PD; k += 32) {
-          float t = 0.f;
-          for (int c = 0; c < C; ++c) t = fmaf(logit[c], Wpp[c * PD + k], t);
-          dEmb[k] = t;
-        }
+        var_readout_tail(emb, Wpp, bpp, C, PD, gt, logit, dEmb, lane);
       }
       for (int idx = tid; idx < nwarps * dp; idx += NT) gFp[idx] = 0.f;
       __syncthreads();
@@ -256,70 +142,21 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
           float g[KW], yh[KW];
 #pragma unroll
           for (int k = 0; k < KW; ++k) g[k] = 0.f;
-          if (l < L) {
-            const int r0 = irp[i], r1 = irp[i + 1], bound = R[l + 1];
-            const float* const dZn = dZ(l + 1);
-            for (int e = r0; e < r1; ++e) {
-              const int j = icol[e];
-              if (j >= bound) break;   // columns are partitioned by level
-              const float ae = a[e];
-#pragma unroll
-              for (int k = 0; k < KW; ++k)
-                if (lane + 32 * k < wout) g[k] = fmaf(ae, dZn[(int64_t)j * VW + lane + 32 * k], g[k]);
-            }
-          }
+          if (l < L) var_gather_back<KW>(irp[i], irp[i + 1], icol, a, dZ(l + 1), wout, R[l + 1], g, lane);   // columns are partitioned by level
 #pragma unroll
           for (int k = 0; k < KW; ++k) {
             if (i == 0 && lane + 32 * k < wout) g[k] += dEmb[hid * (l - 1) + lane + 32 * k];
             yh[k] = Yh(l)[(int64_t)i * VW + lane + 32 * k];
           }
-          if (l < L) {
-            if (kBn) {   // backward of the per-node standardisation: (g - mean(g) - Hb mean(g Hb)) * istd
-              float hb[KW], s1 = 0.f, s2 = 0.f;
-#pragma unroll
-              for (int k = 0; k < KW; ++k) {
-                hb[k] = Hh(l)[(int64_t)i * VW + lane + 32 * k];
-                if (lane + 32 * k < wout) { s1 += g[k]; s2 += g[k] * hb[k]; }
-              }
-              const float m1 = warp_sum(s1) / (float)wout, m2 = warp_sum(s2) / (float)wout, is = istd(l)[i];
-#pragma unroll
-              for (int k = 0; k < KW; ++k) g[k] = lane + 32 * k < wout ? (g[k] - m1 - hb[k] * m2) * is : 0.f;
-            }
-#pragma unroll
-            for (int k = 0; k < KW; ++k) g[k] = yh[k] > 0.f ? g[k] : 0.f;   // relu backward
-          }
-          float sl = 0.f;
-#pragma unroll
-          for (int k = 0; k < KW; ++k) sl += lane + 32 * k < wout ? yh[k] * g[k] : 0.f;
-          const float sdot = warp_sum(sl);
+          if (l < L) var_hidden_backward<kBn, KW>(g, yh, Hh(l) + (int64_t)i * VW, kBn ? istd(l)[i] : 1.f, wout, lane);
+          const float sdot = var_norm_dot<KW>(g, yh, wout, lane);
           const float qi = qn(l)[i];
           __syncwarp();
-#pragma unroll
-          for (int k = 0; k < KW; ++k)
-            if (lane + 32 * k < wout) zs[lane + 32 * k] = (g[k] - yh[k] * sdot) / qi;   // dY: backward of y / max(|y|, eps)
+          var_norm_backward<KW>(g, yh, sdot, qi, wout, zs, lane);   // dY: backward of y / max(|y|, eps)
           __syncwarp();
           // dZ[f] = sum_c dY[c] W[f][c]
-          if (l == 1) {
-            for (int f0 = 0; f0 < d; f0 += 32) {
-              const int f = f0 + lane;
-              float t = 0.f;
-              if (f < d)
-                for (int c = 0; c < wout; ++c) t = fmaf(zs[c], Ws[f * wout + c], t);
-              if (f < d) {
-                gFp[warp * dp + f] = fmaf(t, U[(int64_t)i * dp + f], gFp[warp * dp + f]);   // dL/dsF partial (U = A_m X)
-                dZ1[(int64_t)i * dp + f] = t * sF[f];                                        // kept masked for the edge dots
-              }
-            }
-          } else {
-#pragma unroll
-            for (int k = 0; k < KW; ++k) {
-              const int f = lane + 32 * k;
-              float t = 0.f;
-              if (f < win)
-                for (int c = 0; c < wout; ++c) t = fmaf(zs[c], Ws[f * wout + c], t);
-              dZ(l)[(int64_t)i * VW + f] = f < win ? t : 0.f;
-            }
-          }
+          if (l == 1) var_first_layer_dz(zs, Ws, d, wout, U + (int64_t)i * dp, sF, gFp + warp * dp, dZ1 + (int64_t)i * dp, lane);
+          else var_hidden_dz<KW>(zs, Ws, win, wout, dZ(l) + (int64_t)i * VW, lane);
           __syncwarp();
         }
         __syncthreads();
@@ -335,13 +172,7 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
           const float s = sF[f];
           const float g = s * (1.f - s) * (gsum + hp.c_feat_size / (float)d);
           float mf = mF[f], vf = vF[f], Fv = Fm[f];
-          if (hp.opt == GX_OPT_ADAM) {
-            mf = mf + (g - mf) * hp.one_minus_b1;
-            vf = vf * hp.b2 + hp.one_minus_b2 * g * g;
-            Fv = Fv - step * (mf / (sqrtf(vf) / bc2s + hp.eps));
-          } else {
-            opt_step_other(hp.opt, Fv, g, mf, vf, step);
-          }
+          var_feat_update(hp, g, Fv, mf, vf, step, bc2s);
           mF[f] = mf; vF[f] = vf; Fm[f] = Fv;
           const float sn = sigmoid_f(Fv);
           sF[f] = sn;   // (the edge dots below use dZ1 (.) sF stored in the backward, not this value)
@@ -373,17 +204,8 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
           float2 m2 = mm[p], v2 = vv[p];
           const float gi = Sv.x * (1.f - Sv.x) * (Gd + hp.c_size - ent_over_nn * Mv.x);
           const float gj = Sv.y * (1.f - Sv.y) * (Gd + hp.c_size - ent_over_nn * Mv.y);
-          if (hp.opt == GX_OPT_ADAM) {
-            m2.x = m2.x + (gi - m2.x) * hp.one_minus_b1;
-            m2.y = m2.y + (gj - m2.y) * hp.one_minus_b1;
-            v2.x = v2.x * hp.b2 + hp.one_minus_b2 * gi * gi;
-            v2.y = v2.y * hp.b2 + hp.one_minus_b2 * gj * gj;
-            Mv.x = Mv.x - adam_delta_fast(m2.x, v2.x, step, bc2s, bc2s_inv, hp.eps, ieee);
-            Mv.y = Mv.y - adam_delta_fast(m2.y, v2.y, step, bc2s, bc2s_inv, hp.eps, ieee);
-          } else {
-            opt_step_other(hp.opt, Mv.x, gi, m2.x, v2.x, step);
-            opt_step_other(hp.opt, Mv.y, gj, m2.y, v2.y, step);
-          }
+          var_edge_update(hp, gi, Mv.x, m2.x, v2.x, step, bc2s, bc2s_inv, ieee);
+          var_edge_update(hp, gj, Mv.y, m2.y, v2.y, step, bc2s, bc2s_inv, ieee);
           const float2 Sn = make_float2(sigmoid_fast(Mv.x, ieee), sigmoid_fast(Mv.y, ieee));
           MM[p] = Mv; mm[p] = m2; vv[p] = v2; SS[p] = Sn;
           const float an = 0.5f * (Sn.x + Sn.y);

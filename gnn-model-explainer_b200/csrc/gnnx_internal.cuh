@@ -261,8 +261,31 @@ __host__ __device__ inline GxLayoutG gx_make_layout_graph(int na, int e_d, int n
   return L;
 }
 
+// Global-memory slab of one graph in the graph-mode model-variant kernel (explain_graph_var.cu): every one of the `na` rows with an
+// edge is computed at every layer; hidden-width arrays have row stride vw = 32 * ceil(width / 32).
+struct GxGraphVarLayout {
+  int64_t a, U, dZ1, Yh, H, dZ, q, istd;
+  int64_t total_words;
+};
+__host__ __device__ inline GxGraphVarLayout gx_make_graph_var_layout(int na, int e_d, int d, int L, int vw) {
+  GxGraphVarLayout Lo;
+  const int dp = gx_round_up(d, 4);
+  int64_t o = 0;
+  auto take = [&](int64_t words) { int64_t r = o; o += (words + 3) / 4 * 4; return r; };
+  Lo.a = take(e_d);                           // masked adjacency of every directed edge slot (row-major in the relabelled rows)
+  Lo.U = take((int64_t)na * dp);              // A_m X
+  Lo.dZ1 = take((int64_t)na * dp);            // dL/d(A_m X') (.) sigmoid(feat_mask)
+  Lo.Yh = take((int64_t)L * na * vw);         // per layer: normalised pre-activations
+  Lo.H = take((int64_t)L * na * vw);          // per layer: relu (+ standardisation) output = input of the next layer / the max-pool
+  Lo.dZ = take((int64_t)(L - 1) * na * vw);   // layers 2..L: dL/d(A_m H_{l-1})
+  Lo.q = take((int64_t)L * na);
+  Lo.istd = take((int64_t)L * na);
+  Lo.total_words = o;
+  return Lo;
+}
+
 // ---------------------------------------------------------------------------------------------
-#define GX_CUDA_CHECK(expr)                                                          \
+#define GX_CUDA_CHECK(expr)                                                        \
   do {                                                                               \
     cudaError_t _e = (expr);                                                         \
     if (_e != cudaSuccess) {                                                         \
@@ -341,6 +364,11 @@ cudaError_t gx_launch_graph_plan(const GxGraphBatchDev& gb, int count, GxPlanArr
 cudaError_t gx_launch_explain_graphs(const GxExplainLaunch& cfg, const GxGraphBatchDev& gb, const GxModelDev& m,
                                      const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0, float* out_mask,
                                      float* out_feat, cudaStream_t s);
+cudaError_t gx_launch_explain_graph_var(const GxExplainLaunch& cfg, const GxGraphBatchDev& gb, const GxModelDev& m,
+                                        const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0, float* out_mask,
+                                        float* out_feat, cudaStream_t s);
+int gx_graph_var_smem_bytes(int d, int L, int hid, int emb, int C);
+int gx_graph_var_ctas_per_sm(const GxModelDev& m);
 cudaError_t gx_launch_outer_pairs(const GxHparamsDev& hp, const GxGraphDev& g, const GxPlanArrays& plan, int count,
                                   const float* m0, float* out_mask, const GxExtra& x, cudaStream_t s);
 cudaError_t gx_launch_denoise_topk(const GxPlanArrays& plan, int count, const float* edge_mask, int k2, int cap, float* out_thr,

@@ -96,11 +96,7 @@ class Explainer:
         # utils/train_utils.py:7-23: adam / sgd / rmsprop / adagrad, schedulers none / step / cos
         if getattr(args, "opt", "adam") not in _abi.GX_OPT or getattr(args, "opt_scheduler", "none") not in _abi.GX_SCHED:
             raise ValueError("unknown optimiser / scheduler: %r / %r" % (getattr(args, "opt", None), getattr(args, "opt_scheduler", None)))
-        if graph_mode and getattr(args, "opt", "adam") != "adam":
-            raise NotImplementedError("graph mode builds Adam only (the schedulers work)")
         bn = bool(getattr(model, "bn", False))
-        if bn and graph_mode:
-            raise NotImplementedError("--bn is built for node tasks only")
         if device is None:
             device = int(os.environ.get("LOCAL_RANK", "0")) if torch.cuda.is_available() else 0
         self.engine = Engine(device)
@@ -290,6 +286,8 @@ class Explainer:
         gids = [int(g) for g in graph_indices]
         edge_off = self.engine.plan_graphs(gids)
         hp, init = self._hparams()
+        if self.print_training and self._no_trace:
+            print("(per-epoch trace is not built for --bn / num_gc_layers != 3 / optimisers other than Adam)")
         n = self.engine.batch_n
         m0 = None
         rc = [self.engine.graph_rows_cols(g) for g in gids]

@@ -51,8 +51,8 @@ typedef struct gx_model_dims {
   int32_t flags;       /* GX_MODEL_* bits                               */
 } gx_model_dims;
 #define GX_MODEL_BN 1u /* args.bn (models.py:222-228): per-node standardisation after every hidden ReLU.  num_layers != 3, bn or a
-                        * hidden / output width of 33..128 select the model-variant kernel (node mode, mask optimisation only: no
-                        * trace / optimiser state / grad) */
+                        * hidden / output width of 33..128 select the model-variant kernels (node mode and graph mode, mask
+                        * optimisation only: no trace / optimiser state / grad) */
 
 /* Optimisation hyper-parameters: explainer_main.py:143-167 defaults + ExplainModule.coeffs
  * (explainer/explain.py:624-631) + torch.optim.Adam defaults (utils/train_utils.py:10). */
@@ -206,11 +206,16 @@ int gx_grad_nodes(gx_handle* h, gx_memspace space, float* edge_mask);
 int gx_set_graph_batch_csr(gx_handle* h, int32_t num_graphs, int32_t max_nodes, const int32_t* rowptr,
                            const int32_t* col, const float* feat, int32_t feat_dim, const int32_t* label);
 /* Plans the graphs to explain; edge_off[count+1] (may be NULL) receives the packed slot offsets: the slots of
- * graph t are the entries of its adjacency in row-major order (its slice of the CSR). */
+ * graph t are the entries of its adjacency in row-major order (its slice of the CSR).  Any model gx_set_model accepts:
+ * the default model needs every graph to fit the tuned kernel's shared memory (GX_ERR_UNSUPPORTED otherwise); a model
+ * variant (2 / 4 layers, --bn, widths 33..128) keeps each graph in device memory, bounded by max_nodes <= 4096 only. */
 int gx_plan_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int64_t* edge_off, int64_t* total_edges);
 /* Explainer.explain(node_idx=0, graph_idx=g, graph_mode=True) for every planned graph (model =
  * GcnEncoderGraph: per-layer max-pool readout, models.py:269-316; lap_loss = 0, explain.py:787-788).
- * m0_edges / edge_mask: [total_edges] in `space`, as for gx_explain_nodes. */
+ * m0_edges / edge_mask: [total_edges] in `space`, as for gx_explain_nodes.  Every optimiser / scheduler of gx_hparams.
+ * The default model with Adam runs the tuned kernel (trace and optimiser state supported); model variants and the other
+ * optimisers run the variant kernel: edge_mask / feat_mask only, GX_ERR_UNSUPPORTED for a trace, optimiser state in / out
+ * and GX_INIT_STATE. */
 int gx_explain_graphs(gx_handle* h, const gx_hparams* hp, gx_memspace space, const float* m0_edges,
                       float* edge_mask, float* feat_mask);
 int gx_explain_graphs_ex(gx_handle* h, const gx_hparams* hp, gx_memspace space, const gx_explain_io* io);
