@@ -273,4 +273,22 @@ __device__ __forceinline__ int row_task_gather(int t, int nlong, const IdxT* lli
 }
 
 
+// The kernel arguments every explainer launcher takes from its GxExplainLaunch and call: work queue, pair slabs, model,
+// hyper-parameters, plan and masks.  Args is ExplainArgs or a graph-mode kernel's argument struct.
+template <typename Args>
+inline void fill_queue_args(Args& a, const GxExplainLaunch& cfg, const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan,
+                            const float* m0, float* out_mask, float* out_feat) {
+  a.order = cfg.order; a.ntasks = cfg.ntasks; a.counter = cfg.counter;
+  a.pws = cfg.pws; a.pws_stride_words = cfg.pws_stride_words;
+  a.m = m; a.hp = hp; a.plan = plan;
+  a.m0 = m0; a.out_mask = out_mask; a.out_feat = out_feat;
+}
+inline ExplainArgs explain_args(const GxExplainLaunch& cfg, const GxGraphDev& g, const GxModelDev& m, const GxHparamsDev& hp,
+                                const GxPlanArrays& plan, const float* m0, float* out_mask, float* out_feat) {
+  ExplainArgs a;
+  fill_queue_args(a, cfg, m, hp, plan, m0, out_mask, out_feat);
+  a.g = g; a.gws = cfg.gws; a.gws_stride_words = cfg.gws_stride_words; a.dbg = cfg.dbg; a.x = cfg.x;
+  return a;
+}
+
 }  // namespace

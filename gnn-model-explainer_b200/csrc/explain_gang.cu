@@ -1087,12 +1087,7 @@ int gx_gang_smem_bytes(int d, int hid, int C) {
 cudaError_t gx_launch_explain_gang(const GxExplainLaunch& cfg, const GxGraphDev& g, const GxModelDev& m,
                                    const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                    float* out_mask, float* out_feat, cudaStream_t s) {
-  ExplainArgs args;
-  args.order = cfg.order; args.ntasks = cfg.ntasks; args.counter = cfg.counter;
-  args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
-  args.pws = cfg.pws; args.pws_stride_words = cfg.pws_stride_words;
-  args.g = g; args.m = m; args.hp = hp; args.plan = plan;
-  args.m0 = m0; args.out_mask = out_mask; args.out_feat = out_feat; args.dbg = cfg.dbg; args.x = cfg.x;
+  const ExplainArgs args = explain_args(cfg, g, m, hp, plan, m0, out_mask, out_feat);
   const bool trace = args.x.trace != nullptr;
   if (m.d > 128) return cudaErrorInvalidValue;   // wider inputs: explain_stream.cu
   if (m.hid == 20 && m.emb == 20) return trace ? launch_gang_t<20, 20, true>(cfg, args, s) : launch_gang_t<20, 20, false>(cfg, args, s);

@@ -493,10 +493,8 @@ cudaError_t gx_launch_explain_graphs(const GxExplainLaunch& cfg, const GxGraphBa
                                      const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0, float* out_mask,
                                      float* out_feat, cudaStream_t s) {
   GraphArgs args;
-  args.order = cfg.order; args.ntasks = cfg.ntasks; args.counter = cfg.counter;
-  args.pws = cfg.pws; args.pws_stride_words = cfg.pws_stride_words;
-  args.gb = gb; args.m = m; args.hp = hp; args.plan = plan;
-  args.m0 = m0; args.out_mask = out_mask; args.out_feat = out_feat; args.x = cfg.x;
+  fill_queue_args(args, cfg, m, hp, plan, m0, out_mask, out_feat);
+  args.gb = gb; args.x = cfg.x;
   const bool tr = cfg.x.trace != nullptr;
   auto launch = [&](auto kern) -> cudaError_t {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cfg.smem_bytes);

@@ -308,11 +308,8 @@ cudaError_t gx_launch_explain_graph_var(const GxExplainLaunch& cfg, const GxGrap
                                         const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0, float* out_mask,
                                         float* out_feat, cudaStream_t s) {
   GraphVarArgs args;
-  args.order = cfg.order; args.ntasks = cfg.ntasks; args.counter = cfg.counter;
-  args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
-  args.pws = cfg.pws; args.pws_stride_words = cfg.pws_stride_words;
-  args.gb = gb; args.m = m; args.hp = hp; args.plan = plan;
-  args.m0 = m0; args.out_mask = out_mask; args.out_feat = out_feat;
+  fill_queue_args(args, cfg, m, hp, plan, m0, out_mask, out_feat);
+  args.gb = gb; args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
   const int bytes = gx_graph_var_smem_bytes(m.d, m.L, m.hid, m.emb, m.C);
   return with_graph_var_kernel(m, [&](auto kern) -> cudaError_t {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);

@@ -833,12 +833,7 @@ cudaError_t gx_launch_outer_pairs(const GxHparamsDev& hp, const GxGraphDev& g, c
 cudaError_t gx_launch_explain(const GxExplainLaunch& cfg, const GxGraphDev& g, const GxModelDev& m,
                               const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                               float* out_mask, float* out_feat, cudaStream_t s) {
-  ExplainArgs args;
-  args.order = cfg.order; args.ntasks = cfg.ntasks; args.counter = cfg.counter;
-  args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
-  args.pws = cfg.pws; args.pws_stride_words = cfg.pws_stride_words;
-  args.g = g; args.m = m; args.hp = hp; args.plan = plan;
-  args.m0 = m0; args.out_mask = out_mask; args.out_feat = out_feat; args.dbg = cfg.dbg; args.x = cfg.x;
+  const ExplainArgs args = explain_args(cfg, g, m, hp, plan, m0, out_mask, out_feat);
   if (m.hid == 20 && m.emb == 20) return launch_dims<20, 20>(cfg, args, s);
   if (m.hid == 32 && m.emb == 32) return launch_dims<32, 32>(cfg, args, s);   // any width <= 32, zero-padded by gx_set_model
   return cudaErrorInvalidValue;

@@ -227,12 +227,7 @@ int gx_var_row_stride(int hid, int emb) { return 32 * var_kw(hid, emb); }
 cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, const GxGraphDev& g, const GxModelDev& m,
                                   const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                   float* out_mask, float* out_feat, cudaStream_t s) {
-  ExplainArgs args;
-  args.order = cfg.order; args.ntasks = cfg.ntasks; args.counter = cfg.counter;
-  args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
-  args.pws = cfg.pws; args.pws_stride_words = cfg.pws_stride_words;
-  args.g = g; args.m = m; args.hp = hp; args.plan = plan;
-  args.m0 = m0; args.out_mask = out_mask; args.out_feat = out_feat; args.dbg = cfg.dbg; args.x = cfg.x;
+  const ExplainArgs args = explain_args(cfg, g, m, hp, plan, m0, out_mask, out_feat);
   const int bytes = gx_var_smem_bytes(m.d, m.L, m.hid, m.emb, m.C);
   const int kw = var_kw(m.hid, m.emb);
   auto go = [&](auto kern) -> cudaError_t {

@@ -267,9 +267,11 @@ int64_t gx_launch_count(gx_handle* h);
  * (13 / 27 / 55 / 112 / 226 KB), counts[5] = streaming class, counts[6] = cluster class; smem_bytes (may be NULL) = largest per-CTA
  * shared-memory footprint of each class; *cluster_size = CTAs per task of the cluster class (1 = none). */
 int gx_plan_class_counts(gx_handle* h, int32_t counts[7], int32_t smem_bytes[7], int32_t* cluster_size);
-/* gx_last_class_ms: device timeline of the last gx_explain_nodes call -- per launch class (indices as above) the time its stream reached
- * the launch and the time its kernel finished, in ms after the call's first event; -1 for classes without tasks.  Synchronises like
- * gx_last_explain_ms.  (tools/cluster_study.py; this timeline found the carveout serialisation.) */
+/* gx_last_class_ms: device timeline of the last gx_explain_nodes or gx_explain_graphs call -- per launch class (node mode: indices as
+ * above; graph mode: 0..5 = the footprint classes of gx_plan_graphs) the time its stream reached the launch and the time its kernel
+ * finished, in ms after the call's first event; -1 for classes without tasks, and everywhere for the single whole-batch launch of a
+ * model variant or an optimiser other than Adam.  Synchronises like gx_last_explain_ms.  (tools/cluster_study.py; this timeline
+ * found the carveout serialisation.) */
 int gx_last_class_ms(gx_handle* h, float begin_ms[7], float end_ms[7]);
 int gx_last_explain_ms(gx_handle* h, float* ms);
 

@@ -516,3 +516,26 @@ def test_denoise_topk_properties_random():
             assert np.array_equal(slots[t, :m], keep[:m]) and np.array_equal(out_vals[t, :m], v[keep[:m]])
             assert np.all(slots[t, m:] == -1)
     eng.close()
+
+
+def test_destroy_releases_device_memory():
+    """gx_destroy frees every device buffer the handle allocated: 20 create / plan / explain / destroy cycles, through the
+    shared-memory and the slab kernels, leave the free device memory where it was."""
+    fx = util.load_fixture("rand")
+    nodes = fx.nodes[:4]
+
+    def cycle():
+        for stream in (False, True):
+            eng = util.make_engine(fx)
+            eng.debug_force_stream(stream)
+            plan = eng.plan_nodes(nodes, 3)
+            out = np.zeros(plan.total_edges, np.float32)
+            eng.explain_nodes_host(eng.make_hparams(num_epochs=10), util.golden_m0(fx, plan), out)
+            eng.close()
+
+    cycle()   # loads the kernels the cycle uses: their code stays with the context
+    free0 = torch.cuda.mem_get_info()[0]
+    for _ in range(20):
+        cycle()
+    free1 = torch.cuda.mem_get_info()[0]
+    assert abs(free1 - free0) <= 2 << 20, (free0, free1)
