@@ -40,10 +40,12 @@ def hop_distances(rowptr, col, r, k):
 
 
 def explain_pruned_edges(rowptr, col, X, gt_label, pred_label, r, weights, M0_edges, num_epochs=100, lr=0.1, beta1=0.9,
-                         beta2=0.999, eps=1e-8, c_size=0.005, c_feat=1.0, c_ent=1.0, c_lap=1.0, bn=False, dtype=np.float64):
+                         beta2=0.999, eps=1e-8, c_size=0.005, c_feat=1.0, c_ent=1.0, c_lap=1.0, bn=False, dtype=np.float64, return_F=False):
     """rowptr/col: symmetric local CSR of the k-hop sub-adjacency (k = number of layers), no self loops; X (n,d);
     r = node_idx_new; M0_edges[e] = M0[i,j] at CSR slot e.  Returns the mask value of every CSR slot (the entries
-    of the reference's masked_adj at the nonzeros of sub_adj, row-major) and a dict of counters."""
+    of the reference's masked_adj at the nonzeros of sub_adj, row-major) and a dict of counters; return_F=True also
+    returns the feature-mask parameter F after the last update (num_epochs - 1 updates: sigmoid(F) is the feature mask
+    the kernels return next to the edge mask)."""
     f = dtype
     n, d = X.shape
     X = np.asarray(X, f)
@@ -138,15 +140,17 @@ def explain_pruned_edges(rowptr, col, X, gt_label, pred_label, r, weights, M0_ed
             m_ += (G_ - m_) * f(1 - beta1)
             v_ *= f(beta2); v_ += f(1 - beta2) * G_ * G_
             P_ -= step * m_ / (np.sqrt(v_) / b2s + f(eps))
-    return a, stats
+    return (a, stats, F) if return_F else (a, stats)
 
 
 def explain_pruned_edges_sparse(rowptr, col, X, gt_label, pred_label, r, weights, M0_edges, num_epochs=5, lr=0.1, beta1=0.9, beta2=0.999,
-                                eps=1e-8, c_size=0.005, c_feat=1.0, c_ent=1.0, c_lap=1.0, dtype=np.float64, chunk=1 << 18):
+                                eps=1e-8, c_size=0.005, c_feat=1.0, c_ent=1.0, c_lap=1.0, dtype=np.float64, chunk=1 << 18,
+                                return_F=False):
     """explain_pruned_edges for LARGE subgraphs (BASELINE configs[4]: n ~ 10^5, E_d ~ 6.4e6, d = 128): the same pruned edge-list
     mathematics with scipy.sparse SpMM and chunked SDDMM instead of np.add.at over (E, width) temporaries.  3-layer / no-bn model
     (what the streaming kernel implements).  tests/test_oracle.py pins it to explain_pruned_edges (and through it to the dense closed
-    form and the reference) on small graphs; bench.py --workload c5 uses it to check the streaming kernel at full scale."""
+    form and the reference) on small graphs; bench.py --workload c5 uses it to check the streaming kernel at full scale.
+    return_F=True: returns (a, F) with F the feature-mask parameter after the last update, as explain_pruned_edges does."""
     import scipy.sparse as sp
     f = dtype
     n, d = X.shape
@@ -230,4 +234,4 @@ def explain_pruned_edges_sparse(rowptr, col, X, gt_label, pred_label, r, weights
             m_ += (G_ - m_) * f(1 - beta1)
             v_ *= f(beta2); v_ += f(1 - beta2) * G_ * G_
             P_ -= step * m_ / (np.sqrt(v_) / b2s + f(eps))
-    return a
+    return (a, F) if return_F else a
