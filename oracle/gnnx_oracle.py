@@ -140,6 +140,48 @@ def draw_m0(n, seed=None):
 
 
 # ----------------------------------------------------------------------------------------------
+# The kernels' device init (GX_INIT_PHILOX, csrc/explain_common.cuh): Philox4x32-10 (Salmon et al. 2011,
+# the Random123 philox4x32 with 10 rounds) and one Box-Muller normal per (seed, key, slot)
+# ----------------------------------------------------------------------------------------------
+_MASK32 = np.uint64(0xFFFFFFFF)
+
+
+def philox4x32_10(ctr, key):
+    """ctr: 4 uint32 words (scalars or equal-length arrays), key: 2 uint32 words -> the 4 output words (uint32 arrays)."""
+    c = [np.asarray(x, dtype=np.uint64) & _MASK32 for x in ctr]
+    k0, k1 = (np.asarray(x, dtype=np.uint64) & _MASK32 for x in key)
+    for _ in range(10):
+        p0 = np.uint64(0xD2511F53) * c[0]
+        p1 = np.uint64(0xCD9E8D57) * c[2]
+        hi0, lo0 = p0 >> np.uint64(32), p0 & _MASK32
+        hi1, lo1 = p1 >> np.uint64(32), p1 & _MASK32
+        c = [hi1 ^ c[1] ^ k0, lo1, hi0 ^ c[3] ^ k1, lo0]
+        k0 = (k0 + np.uint64(0x9E3779B9)) & _MASK32
+        k1 = (k1 + np.uint64(0xBB67AE85)) & _MASK32
+    return [x.astype(np.uint32) for x in c]
+
+
+def philox_normal(seed, key, slot):
+    """N(0,1) the kernels draw for (seed, key, slot), in float64: counter (slot, key, 0x67, 0x6e78), key (seed lo, seed hi),
+    Box-Muller on the top 24 bits of the first two output words."""
+    slot = np.asarray(slot, dtype=np.uint64)
+    seed = int(seed)
+    r = philox4x32_10((slot, np.full_like(slot, key), np.full_like(slot, 0x67), np.full_like(slot, 0x6E78)),
+                      (seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF))
+    u1 = ((r[0] >> np.uint32(8)).astype(np.float64) + 0.5) / 16777216.0
+    u2 = ((r[1] >> np.uint32(8)).astype(np.float64) + 0.5) / 16777216.0
+    return np.sqrt(-2.0 * np.log(u1)) * np.cos(2.0 * np.pi * u2)
+
+
+def philox_m0(seed, key, num_slots, n):
+    """The M0 entries GX_INIT_PHILOX draws for one task, float64 [num_slots], slot = position in the task's edge arrays:
+    1 + sqrt(2/n) * philox_normal(seed, key, slot), i.e. N(1, gain('relu')^2 * 2/(n+n)) as construct_edge_mask draws.
+    Node mode: key = the explained node's id, n = its neighbourhood size, slots in canonical (row-major) order.
+    Graph mode: key = the graph id, n = max_nodes (the padded size), slots in the order of the graph's CSR."""
+    return 1.0 + math.sqrt(2.0 / n) * philox_normal(seed, key, np.arange(num_slots))
+
+
+# ----------------------------------------------------------------------------------------------
 # a3..a12, line-by-line port: dense tensors + autograd + torch.optim.Adam
 # ----------------------------------------------------------------------------------------------
 
@@ -192,13 +234,14 @@ def weights_to_torch(weights, requires_grad=True):
 
 
 def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0,
-                        hp=None, graph_mode=False, trace=None, bn=False):
+                        hp=None, graph_mode=False, trace=None, bn=False, return_feat=False):
     """Port of Explainer.explain's optimisation (explain.py:97-146,209-211) with
     ExplainModule.{_masked_adj,forward,loss,mask_density} (explain.py:665-808) inlined.
 
     sub_adj (n,n) 0/1; sub_feat (n,d); gt_label = label[0][node_idx] (node) or the graph label;
     pred_label (n,) int = argmax(pred[nbrs]) (node mode; unused in graph mode); M0 (n,n) float32.
-    Returns the (n,n) float64 array the reference returns (masked_adj[0] * sub_adj)."""
+    Returns the (n,n) float64 array the reference returns (masked_adj[0] * sub_adj); return_feat=True also
+    returns sigmoid(feat_mask) as the last epoch's forward used it (after num_epochs - 1 updates), float64 (d,)."""
     import torch
     hp = hp or default_hparams()
     W = weights if isinstance(weights, dict) and "conv_w" in weights else weights_to_torch(weights)
@@ -249,6 +292,7 @@ def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
         m = torch.sigmoid(mask)                                                 # explain.py:756-757
         size_loss = hp.size * torch.sum(m)                                      # explain.py:760
         fm = torch.sigmoid(feat_mask)
+        fm_used = fm.detach()
         feat_size_loss = hp.feat_size * torch.mean(fm)                          # explain.py:766
         mask_ent = -m * torch.log(m) - (1 - m) * torch.log(1 - m)               # explain.py:769
         mask_ent_loss = hp.ent * torch.mean(mask_ent)                           # explain.py:770
@@ -276,7 +320,10 @@ def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
                                   size_edges=float(hp.size * torch.sum(m_used[on])), size_off=float(hp.size * torch.sum(m_used[~on])),
                                   ent_edges=float(hp.ent * torch.sum(ent_used[on]) / adj.numel()),
                                   ent_off=float(hp.ent * torch.sum(ent_used[~on]) / adj.numel())))
-    return masked_adj[0].detach().numpy() * np.asarray(sub_adj, dtype=np.float64)   # explain.py:209-211
+    out = masked_adj[0].detach().numpy() * np.asarray(sub_adj, dtype=np.float64)   # explain.py:209-211
+    if return_feat:
+        return out, fm_used.numpy().astype(np.float64)
+    return out
 
 
 # ----------------------------------------------------------------------------------------------
@@ -411,7 +458,8 @@ def explain_closed_form(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
             P -= step * m_ / (np.sqrt(v_) / b2s + f(hp.eps))
     out = a.astype(np.float64) * np.asarray(sub_adj, dtype=np.float64)
     if return_state:
-        return out, dict(M=M, F=F, gM=gM, gF=gF, p=p)
+        # M, F and the Adam moments after num_epochs updates; init_state=dict(m=mM, v=vM, feat=(F, mF, vF), step=...) resumes from them
+        return out, dict(M=M, F=F, gM=gM, gF=gF, p=p, mM=mM, vM=vM, mF=mF, vF=vF)
     return out
 
 

@@ -12,7 +12,7 @@ import gnnx
 import gnnx_oracle as O
 import util
 from gnnx import _abi
-from test_oracle_graph_variants import BASE_KEYS, MODEL_TAGS, model_of
+from test_oracle_graph_variants import BASE_KEYS, MODEL_TAGS, OPT_TAGS, dense_m0, model_of
 
 pytestmark = pytest.mark.gpu
 OPT_CASES = {"sgd": dict(opt=1), "rmsprop": dict(opt=2), "adagrad": dict(opt=3),
@@ -37,13 +37,14 @@ def _engine(w, L, bn, adj, feat, label):
     return eng
 
 
-def _run(eng, gids, m0_of, epochs, **over):
+def _run(eng, gids, m0_of, epochs, with_feat=False, **over):
     edge_off = eng.plan_graphs(gids)
     m0 = np.concatenate([m0_of(g) for g in gids]).astype(np.float32)
     assert len(m0) == edge_off[-1]
     out = np.zeros(len(m0), np.float32)
-    eng.explain_graphs_host(eng.make_hparams(num_epochs=epochs, **over), m0, out)
-    return edge_off, out
+    fm = np.zeros((len(gids), eng.input_dim), np.float32) if with_feat else None
+    eng.explain_graphs_host(eng.make_hparams(num_epochs=epochs, **over), m0, out, fm)
+    return (edge_off, out, fm) if with_feat else (edge_off, out)
 
 
 @pytest.mark.parametrize("tag", MODEL_TAGS + list(OPT_CASES))
@@ -54,12 +55,22 @@ def test_graph_variants_match_reference_golden(gv, gg, tag):
         (w, L, bn), over = model_of(gv, tag), {}
     eng = _engine(w, L, bn, gg["adj"], gg["feat"], gg["label"])
     gids = list(range(int(gg["num_graphs"])))
-    edge_off, out = _run(eng, gids, lambda g: gg["g%d_m0" % g], int(gv["num_epochs"]), **over)
+    E = int(gv["num_epochs"])
+    edge_off, out, fm = _run(eng, gids, lambda g: gg["g%d_m0" % g], E, with_feat=True, **over)
     eng.close()
     for t, g in enumerate(gids):
         err = util.rel_l2(out[edge_off[t]:edge_off[t + 1]], gv["%s_g%d_mask" % (tag, g)])
         tol = max(1e-4, 3 * float(gv[tag + "_spread"][g]))
         assert err <= tol, (tag, g, err, tol)
+        A, M0 = gg["adj"][g].astype(np.float64), dense_m0(gg, g)
+        args = (A, gg["feat"][g], int(gg["label"][g]), None, 0, w, M0)
+        if tag in OPT_CASES:   # no closed form for these optimisers: the port's feature mask, at 30 x the reference's own spread
+            _, ref_fm = O.explain_dense_torch(*args, hp=O.default_hparams(num_epochs=E, **OPT_TAGS[tag]), graph_mode=True, return_feat=True)
+            assert np.abs(ref_fm - 0.5).max() > 1e-3
+            ferr = np.abs(fm[t] - ref_fm).max()
+            assert ferr <= max(2e-4, 30 * float(gv[tag + "_spread"][g])), (tag, g, ferr)
+        else:
+            util.check_graph_masks(A, gg["feat"][g], gg["label"][g], w, M0, E, None, fm[t], np.nonzero(A), bn=bn)
 
 
 def _random_model(rng, L, bn, hid, emb, d, C, bias):
@@ -84,16 +95,8 @@ def _check_against_port(eng, w, L, bn, adj, feat, label, gids, epochs, seed):
     edge_off = eng.plan_graphs(gids)
     out = np.zeros(int(edge_off[-1]), np.float32)
     eng.explain_graphs_host(eng.make_hparams(num_epochs=epochs), np.concatenate([dense[g][rc[g]] for g in gids]).astype(np.float32), out, fm)
-    hp = O.default_hparams(num_epochs=epochs)
     for t, g in enumerate(gids):
-        A = adj[g].astype(np.float64)
-        ref = O.explain_dense_torch(A, feat[g], int(label[g]), None, 0, w, dense[g], hp=hp, graph_mode=True, bn=bn)
-        c64 = O.explain_closed_form(A, feat[g], int(label[g]), None, 0, w, dense[g], hp=hp, graph_mode=True, bn=bn)
-        assert np.isfinite(ref[rc[g]]).all(), g   # (the reference's entropy term can overflow to NaN on some random models)
-        tol = max(1e-4, 3 * O.rel_l2(c64[rc[g]], ref[rc[g]]))
-        err = O.rel_l2(out[edge_off[t]:edge_off[t + 1]], ref[rc[g]])
-        assert err <= tol, (g, err, tol)
-    assert np.isfinite(fm).all() and (fm > 0).all() and (fm < 1).all()
+        util.check_graph_masks(adj[g], feat[g], label[g], w, dense[g], epochs, out[edge_off[t]:edge_off[t + 1]], fm[t], rc[g], bn=bn)
 
 
 @pytest.mark.parametrize("seed,L,bn,hid,emb,d,C,bias", [(1, 3, True, 64, 48, 14, 3, "positive"), (2, 2, False, 33, 40, 100, 4, "none"),
@@ -148,17 +151,28 @@ def test_order_and_batch_independence(gv, gg):
 
 
 def test_philox_init_equals_the_tuned_kernel(gg):
-    """GX_INIT_PHILOX draws the same M0 in both graph kernels: at num_epochs = 1 (the mask before any update) an SGD run (variant
-    kernel) equals an Adam run (tuned kernel)."""
+    """GX_INIT_PHILOX in both graph kernels draws the M0 of its host restatement (gnnx_oracle.philox_m0: key = graph id, slot = position
+    in the graph's CSR, std sqrt(2 / max_nodes)): at num_epochs = 1 (the mask before any update) an SGD run (variant kernel) and an Adam
+    run (tuned kernel) both return (sigmoid(M0_ij) + sigmoid(M0_ji)) / 2."""
     eng = _engine({k: gg[k] for k in BASE_KEYS}, 3, False, gg["adj"], gg["feat"], gg["label"])
-    edge_off = eng.plan_graphs(list(range(int(gg["num_graphs"]))))
+    gids = list(range(int(gg["num_graphs"])))
+    edge_off = eng.plan_graphs(gids)
+    n, seed = int(gg["max_nodes"]), 1234 + (3 << 32)      # the seed's high word keys the generator too
+    want = []
+    for t, g in enumerate(gids):
+        r, c = eng.graph_rows_cols(g)
+        S = np.full((n, n), np.nan)
+        S[r, c] = 1 / (1 + np.exp(-O.philox_m0(seed, g, len(r), n)))
+        want.append((S[r, c] + S[c, r]) / 2)
+    want = np.concatenate(want)
     res = []
     for opt in (0, 1):
         out = np.zeros(int(edge_off[-1]), np.float32)
-        eng.explain_graphs_host(eng.make_hparams(num_epochs=1, init=_abi.GX_INIT_PHILOX, seed=1234, opt=opt), None, out)
+        eng.explain_graphs_host(eng.make_hparams(num_epochs=1, init=_abi.GX_INIT_PHILOX, seed=seed, opt=opt), None, out)
         res.append(out)
     eng.close()
     assert np.abs(res[0] - res[1]).max() <= 1e-6
+    assert np.abs(res[0] - want).max() <= 1e-6 and np.abs(res[1] - want).max() <= 1e-6
     assert np.isfinite(res[0]).all() and 0.3 < res[0].mean() < 0.95
 
 

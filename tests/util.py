@@ -65,6 +65,30 @@ def assert_per_node(errs, name, epochs):
     return tol
 
 
+def check_graph_masks(A, X, label, w, M0, epochs, edge_mask, feat_mask, rc, bn=False, edge_tol=None):
+    """One graph-mode result (Adam) against the CPU oracle.  Edge masks (slot order rc = (rows, cols)) vs the line-by-line port at
+    max(1e-4, 3 x dis), dis = rel-L2(fp64 closed form, port): how far two faithful restatements of the same trajectory land apart
+    (edge_tol overrides the bound; edge_mask None: not compared).  The feature mask vs sigmoid(F) of the fp64 closed form after epochs - 1 updates (what the
+    kernels return) at max(2e-4, 30 x dis).  Returns dis."""
+    import gnnx_oracle as O
+    r, c = rc
+    args = (np.asarray(A, np.float64), X, int(label), None, 0, w, M0)
+    port = O.explain_dense_torch(*args, hp=O.default_hparams(num_epochs=epochs), graph_mode=True, bn=bn)
+    c64 = O.explain_closed_form(*args, hp=O.default_hparams(num_epochs=epochs), graph_mode=True, bn=bn)
+    assert np.isfinite(port[r, c]).all()   # (the reference's entropy term can overflow to NaN on some random models)
+    dis = rel_l2(c64[r, c], port[r, c])
+    if edge_mask is not None:
+        err = rel_l2(edge_mask, port[r, c])
+        tol = max(1e-4, 3 * dis) if edge_tol is None else edge_tol
+        assert err <= tol, ("edge mask", err, tol)
+    _, st = O.explain_closed_form(*args, hp=O.default_hparams(num_epochs=epochs - 1), graph_mode=True, bn=bn, return_state=True)
+    sF = 1 / (1 + np.exp(-st["F"]))
+    assert np.abs(sF - 0.5).max() > 1e-3      # F has moved: the comparison below can fail
+    ferr = float(np.abs(np.asarray(feat_mask, np.float64) - sF).max())
+    assert ferr <= max(2e-4, 30 * dis), ("feature mask", ferr, max(2e-4, 30 * dis))
+    return dis
+
+
 def rel_l2(a, b):
     a = np.asarray(a, np.float64).ravel()
     b = np.asarray(b, np.float64).ravel()
