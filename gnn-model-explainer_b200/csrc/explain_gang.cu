@@ -19,6 +19,7 @@
 // Phases per epoch (gang barrier each): F0 | F1 | F2 | S (every CTA, redundantly) | B2 | B1 | B0s | B0d | P.
 // Supported: feature widths d <= 128 (wider inputs keep explain_stream.cu), hidden width 20 or 32.
 #include "explain_common.cuh"
+#include "mma_tf32.cuh"
 
 namespace {
 
@@ -105,19 +106,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void tma_load_1d(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t l2_policy) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(l2_policy) : "memory");
 }
-
-// ------------------------------------------------------------------------------------------------ tensor cores (3xTF32)
-__device__ __forceinline__ uint32_t tf32_of(float x) { uint32_t r; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x)); return r; }
-__device__ __forceinline__ void tf32_split(float x, uint32_t& hi, uint32_t& lo) {
-  hi = tf32_of(x);
-  lo = tf32_of(x - __uint_as_float(hi));
-}
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-// 3xTF32: (ahi + alo)(bhi + blo) without the lo*lo term = alo*bhi + ahi*blo (small) + ahi*bhi (big), each an mma_tf32 (see the callers)
 
 __device__ __forceinline__ float4 ldcg4(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
 

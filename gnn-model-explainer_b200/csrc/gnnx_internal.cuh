@@ -284,8 +284,40 @@ __host__ __device__ inline GxGraphVarLayout gx_make_graph_var_layout(int na, int
   return Lo;
 }
 
+// Global-memory slab of one task in the unconstrained kernel (explain_dense.cu): the dense n x n state and the per-layer activations of
+// all n rows.  Hc / dZc hold, per row, the layer inputs X = H_0, H_1 .. H_L and the matching dL/d(A_m H_{l-1}) side by side: column
+// offset 0 for X / dZ_1 (width d), off1 + (l - 1) vw for H_l / dZ_{l+1} (vw = 32 * ceil(width / 32)), so that every pair gradient
+// sum_l dZ_l H_{l-1}^T is ONE product dZc Hc^T over the first k_pair columns; padding columns stay zero.
+constexpr int GX_DENSE_MAX_N = 4096;   // 16.7 M mask parameters per task, the bound of graph mode's max_nodes
+struct GxDenseLayout {
+  int64_t M, m, v, a, G, Hc, dZc, Z, Yh, q, istd;
+  int64_t total_words;
+  int off1, kh, k_pair, zw;
+};
+__host__ __device__ inline GxDenseLayout gx_make_dense_layout(int n, int d, int L, int vw) {
+  GxDenseLayout Lo;
+  Lo.off1 = gx_round_up(d, 8);
+  Lo.k_pair = Lo.off1 + (L - 1) * vw;
+  Lo.kh = Lo.k_pair + vw;
+  Lo.zw = Lo.off1 > vw ? Lo.off1 : vw;
+  const int64_t nn = (int64_t)n * n;
+  int64_t o = 0;
+  auto take = [&](int64_t words) { int64_t r = o; o += (words + 3) / 4 * 4; return r; };
+  Lo.M = take(nn); Lo.m = take(nn); Lo.v = take(nn);   // mask parameter and optimiser state of every directed entry (i, j) at i * n + j
+  Lo.a = take(nn);                                      // masked adjacency sym(sigmoid(M)) (.) (1 - I)
+  Lo.G = take(nn);                                      // pair-gradient product dZc Hc^T
+  Lo.Hc = take((int64_t)n * Lo.kh);
+  Lo.dZc = take((int64_t)n * Lo.kh);
+  Lo.Z = take((int64_t)n * Lo.zw);                      // output of the current aggregation product
+  Lo.Yh = take((int64_t)L * n * vw);                    // per layer: normalised pre-activations
+  Lo.q = take((int64_t)L * n);
+  Lo.istd = take((int64_t)L * n);
+  Lo.total_words = o;
+  return Lo;
+}
+
 // ---------------------------------------------------------------------------------------------
-#define GX_CUDA_CHECK(expr)                                                        \
+#define GX_CUDA_CHECK(expr)                                                      \
   do {                                                                               \
     cudaError_t _e = (expr);                                                         \
     if (_e != cudaSuccess) {                                                         \
@@ -369,6 +401,22 @@ cudaError_t gx_launch_explain_graph_var(const GxExplainLaunch& cfg, const GxGrap
                                         float* out_feat, cudaStream_t s);
 int gx_graph_var_smem_bytes(int d, int L, int hid, int emb, int C);
 int gx_graph_var_ctas_per_sm(const GxModelDev& m);
+// explain_dense.cu: Explainer.explain(..., unconstrained=True), node mode (graph_mode 0, g) or graph mode (gb); m0 / out_dense are dense
+// (dense_off[t] = the offset of task t's n_t^2 block), out_mask holds the sub-adjacency slots, x.trace / x.trace_pred optional.
+struct GxDenseIo {
+  const int64_t* dense_off;
+  const float* m0;
+  float* out_mask;
+  float* out_dense;
+  float* trace;
+  float* trace_pred;
+  int32_t epochs;
+};
+cudaError_t gx_launch_explain_dense(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
+                                    const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan, const GxDenseIo& io,
+                                    cudaStream_t s);
+int gx_dense_smem_bytes(int d, int L, int hid, int emb, int C);
+int gx_dense_ctas_per_sm(const GxModelDev& m);
 cudaError_t gx_launch_outer_pairs(const GxHparamsDev& hp, const GxGraphDev& g, const GxPlanArrays& plan, int count,
                                   const float* m0, float* out_mask, const GxExtra& x, cudaStream_t s);
 cudaError_t gx_launch_denoise_topk(const GxPlanArrays& plan, int count, const float* edge_mask, int k2, int cap, float* out_thr,

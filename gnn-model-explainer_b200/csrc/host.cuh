@@ -100,6 +100,7 @@ struct gx_handle {
   DevBuf d_pws, d_gws, d_adam, d_m0, d_out, d_feat, d_dense_off, d_dense, d_rows;
   DevBuf d_trace, d_trpred, d_trouter, d_min, d_vin, d_fsin, d_Mout, d_mout, d_vout, d_fsout, d_m0dense, d_offedge;   // gx_explain_io staging (GX_HOST)
   DevBuf d_dn_thr, d_dn_cnt, d_dn_slots, d_dn_vals, d_us, d_gang, d_fwd;
+  DevBuf d_uorder, d_mdense;   // unconstrained.cu: its work order (the plan's d_order stays for the constrained kernels), mask_dense staging
   GxComm* comm = nullptr;
   int32_t label_min = 0, label_max = 0, pred_min = 0, pred_max = 0;   // ranges of the uploaded labels (checked against num_classes at plan time)
   bool has_label = false;

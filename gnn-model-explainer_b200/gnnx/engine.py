@@ -252,6 +252,21 @@ class Engine:
         fn = self._lib.gx_explain_graphs_ex if graphs else self._lib.gx_explain_nodes_ex
         _abi.check(fn(self._h, C.byref(hp), _abi.GX_HOST, C.byref(io)))
 
+    def explain_nodes_unconstrained(self, hp, m0_dense, edge_mask_out, mask_dense_out=None, trace=None, trace_pred=None):
+        """Explainer.explain(..., unconstrained=True) for every planned node (gx_explain_nodes_unconstrained), host (numpy) buffers:
+        m0_dense float32 [sum_t n_t^2] (None with GX_INIT_PHILOX); edge_mask_out float32 [total_edges]; mask_dense_out float32
+        [sum_t n_t^2]; trace float32 (count, num_epochs, 8); trace_pred float32 (count, num_epochs, C)."""
+        self._unconstrained(self._lib.gx_explain_nodes_unconstrained, hp, m0_dense, edge_mask_out, mask_dense_out, trace, trace_pred)
+
+    def explain_graphs_unconstrained(self, hp, m0_dense, edge_mask_out, mask_dense_out=None, trace=None, trace_pred=None):
+        """The same for every planned graph (gx_explain_graphs_unconstrained): n_t = max_nodes, edge_mask_out at the graphs' CSR slots."""
+        self._unconstrained(self._lib.gx_explain_graphs_unconstrained, hp, m0_dense, edge_mask_out, mask_dense_out, trace, trace_pred)
+
+    def _unconstrained(self, fn, hp, m0_dense, edge_mask_out, mask_dense_out, trace, trace_pred):
+        m0 = None if m0_dense is None else _f32c(m0_dense)
+        _abi.check(fn(self._h, C.byref(hp), _abi.GX_HOST, _np_ptr(m0), _np_ptr(edge_mask_out), _np_ptr(mask_dense_out),
+                      _np_ptr(trace), _np_ptr(trace_pred)))
+
     def offedge_regularisers(self, hp, m0_dense):
         """(count, num_epochs, 2) float64: per epoch (sum sigmoid(M), sum H(sigmoid(M))) over the mask entries outside the
         sub-adjacency -- the part of the reference's printed loss that never influences the result (gx_offedge_regularisers)."""

@@ -230,8 +230,6 @@ class Explainer:
     def _explain_batch(self, node_indices, graph_idx=0, model="exp", unconstrained=False):
         if model not in ("exp", "grad"):
             raise NotImplementedError("model=%r (att) is not built" % model)
-        if unconstrained:
-            raise NotImplementedError("unconstrained=True is not built")
         self._select_graph(graph_idx)
         nodes = [int(i) for i in node_indices]
         plan = self.engine.plan_nodes(nodes, self.n_hops)
@@ -239,9 +237,20 @@ class Explainer:
         if model == "grad":        # explain.py:125-133: one backward to the adjacency, no mask parameters (the reference still
             if self._hparams()[1] == "torch":      # constructs an ExplainModule per node, i.e. consumes n^2 normals: keep the RNG in step)
                 self._draw_m0(plan)
-            self.engine.grad_nodes_host(edge_mask)
+            self.engine.grad_nodes_host(edge_mask)     # (unconstrained is ignored here, as in the reference)
             return plan, edge_mask
         hp, init = self._hparams()
+        if unconstrained:
+            # explain.py:688-692: the dense mask drives the forward, so every one of the n^2 normals of M0 is a parameter
+            m0 = np.concatenate([D.reshape(-1) for D in self._draw_m0(plan, keep_dense=True)[1]]) if init == "torch" else None
+            if not self.print_training:
+                self.engine.explain_nodes_unconstrained(hp, m0, edge_mask)
+                return plan, edge_mask
+            trace = np.zeros((plan.count, hp.num_epochs, _abi.GX_TRACE_COLS), np.float32)
+            pred = np.zeros((plan.count, hp.num_epochs, self.engine.num_classes), np.float32)
+            self.engine.explain_nodes_unconstrained(hp, m0, edge_mask, trace=trace, trace_pred=pred)
+            self.last_trace = self._print_trace(plan, hp, trace, pred, None)    # the kernel's loss covers all n^2 entries
+            return plan, edge_mask
         if not self.print_training or self._no_trace:
             if self.print_training:
                 print("(per-epoch trace is not built for --bn / num_gc_layers != 3 / optimisers other than Adam)")
@@ -282,23 +291,29 @@ class Explainer:
         return fname
 
     # ---------------------------------------------------------------- public API
-    def _explain_graph_batch(self, graph_indices):
+    def _explain_graph_batch(self, graph_indices, unconstrained=False):
         gids = [int(g) for g in graph_indices]
         edge_off = self.engine.plan_graphs(gids)
         hp, init = self._hparams()
-        if self.print_training and self._no_trace:
+        if self.print_training and self._no_trace and not unconstrained:
             print("(per-epoch trace is not built for --bn / num_gc_layers != 3 / optimisers other than Adam)")
         n = self.engine.batch_n
         m0 = None
         rc = [self.engine.graph_rows_cols(g) for g in gids]
         if init == "torch":
-            m0 = np.empty(int(edge_off[-1]), dtype=np.float32)
+            m0 = np.empty(n * n * len(gids) if unconstrained else int(edge_off[-1]), dtype=np.float32)
             std = torch.nn.init.calculate_gain("relu") * math.sqrt(2.0 / (n + n))
             for t, (rows, cols) in enumerate(rc):
                 M = torch.FloatTensor(n, n).normal_(1.0, std).numpy()      # explain.py:645-652, n = padded size
-                m0[edge_off[t]:edge_off[t + 1]] = M[rows, cols]
+                if unconstrained:
+                    m0[t * n * n:(t + 1) * n * n] = M.reshape(-1)
+                else:
+                    m0[edge_off[t]:edge_off[t + 1]] = M[rows, cols]
         edge_mask = np.empty(int(edge_off[-1]), dtype=np.float32)
-        self.engine.explain_graphs_host(hp, m0, edge_mask)
+        if unconstrained:
+            self.engine.explain_graphs_unconstrained(hp, m0, edge_mask)
+        else:
+            self.engine.explain_graphs_host(hp, m0, edge_mask)
         out = []
         for t, (rows, cols) in enumerate(rc):
             D = np.zeros((n, n), dtype=np.float64)
@@ -323,9 +338,9 @@ class Explainer:
         if graph_mode or self.graph_mode:
             if not self.graph_mode:
                 raise ValueError("Explainer was not constructed with graph_mode=True")
-            if model != "exp" or unconstrained:
-                raise NotImplementedError("only model='exp', unconstrained=False are built")
-            masked_adj = self._explain_graph_batch([graph_idx])[0]
+            if model != "exp":
+                raise NotImplementedError("only model='exp' is built in graph mode")
+            masked_adj = self._explain_graph_batch([graph_idx], unconstrained)[0]
             fname = self._save(masked_adj, node_idx)
             if self.print_training:
                 print("Saved adjacency matrix to ", fname)

@@ -220,6 +220,25 @@ int gx_explain_graphs(gx_handle* h, const gx_hparams* hp, gx_memspace space, con
                       float* edge_mask, float* feat_mask);
 int gx_explain_graphs_ex(gx_handle* h, const gx_hparams* hp, gx_memspace space, const gx_explain_io* io);
 
+/* ---- unconstrained masks: Explainer.explain(..., unconstrained=True) (explain.py:97-146,209-211; ExplainModule.forward
+ * explain.py:688-692) for every planned node (after gx_plan_nodes) or graph (after gx_plan_graphs).  The forward sees the dense
+ * mask sym(sigmoid(M)) * (1 - I), NOT multiplied by the sub-adjacency, and the unmasked features; the loss (explain.py:740-808) is
+ * evaluated on that dense matrix.  One CTA per task keeps its n^2 mask parameters in device memory: n = the k-hop set (node mode)
+ * or max_nodes (graph mode), n > 4096 gives GX_ERR_UNSUPPORTED.  Every model and optimiser / scheduler of gx_hparams;
+ * GX_INIT_STATE gives GX_ERR_UNSUPPORTED.  All buffers in `space`:
+ *   m0_dense    [sum_t n_t^2] GX_INIT_M0: the full (n_t, n_t) M0 of every task, task after task (GX_INIT_PHILOX: NULL; the draw uses
+ *               slot = i * n_t + j)
+ *   edge_mask   [total_edges] out: masked_adj at the sub-adjacency slots (node mode: the sub_col slots; graph mode: the graph's
+ *               CSR slots), i.e. the array the reference returns, masked_adj[0] * sub_adj
+ *   mask_dense  optional [sum_t n_t^2] out: the whole symmetric mask, zero diagonal
+ *   trace       optional [count*num_epochs*GX_TRACE_COLS] out: the GX_TR_* columns; loss, size, entropy and Laplacian cover all n^2
+ *               entries (no gx_offedge_regularisers needed), the density is mask_density()'s constrained one (explain.py:680-683)
+ *   trace_pred  optional [count*num_epochs*num_classes] out, needs trace */
+int gx_explain_nodes_unconstrained(gx_handle* h, const gx_hparams* hp, gx_memspace space, const float* m0_dense,
+                                   float* edge_mask, float* mask_dense, float* trace, float* trace_pred);
+int gx_explain_graphs_unconstrained(gx_handle* h, const gx_hparams* hp, gx_memspace space, const float* m0_dense,
+                                    float* edge_mask, float* mask_dense, float* trace, float* trace_pred);
+
 /* Expands packed edge masks to the dense (n_t, n_t) float64 arrays Explainer.explain returns
  * (explain.py:209-221), task after task, into out (sum_t n_t^2 doubles, `space`). */
 int gx_densify(gx_handle* h, gx_memspace space, const float* edge_mask, double* out);

@@ -1,0 +1,228 @@
+"""dense_oracle.py -- CPU restatements of Explainer.explain(..., unconstrained=True).  TEST INFRASTRUCTURE ONLY.
+
+With unconstrained=True (ExplainModule.forward, explain.py:688-692) the forward's adjacency is the DENSE mask
+sym(sigmoid(M)) * (1 - I), not multiplied by the sub-adjacency, and the features are not masked.  Two restatements, as for the
+constrained path in oracle/gnnx_oracle.py (whose helpers they reuse):
+  * explain_dense_torch  -- line-by-line port (dense tensors, torch autograd, torch.optim), bit-exact to the unmodified reference
+                            (tests/golden/unconstrained_golden.npz, tools/gen_unconstrained_golden.py); the CPU baseline.
+  * explain_closed_form  -- hand-derived forward / backward in numpy (fp64 or fp32): the specification csrc/explain_dense.cu implements.
+Both return the (n, n) float64 array the reference returns, masked_adj[0] * sub_adj (explain.py:209-211).
+"""
+import math
+
+import numpy as np
+
+import gnnx_oracle as O
+
+
+def _optimizer(hp, params):
+    """utils/train_utils.py:7-23 (build_optimizer; explain.py:622)."""
+    import torch
+    if hp.opt == "adam":
+        opt = torch.optim.Adam(params, lr=hp.lr, betas=(hp.beta1, hp.beta2), eps=hp.eps)
+    elif hp.opt == "sgd":
+        opt = torch.optim.SGD(params, lr=hp.lr, momentum=0.95)
+    elif hp.opt == "rmsprop":
+        opt = torch.optim.RMSprop(params, lr=hp.lr)
+    elif hp.opt == "adagrad":
+        opt = torch.optim.Adagrad(params, lr=hp.lr)
+    else:
+        raise ValueError(hp.opt)
+    sched = None
+    if hp.opt_scheduler == "step":
+        sched = torch.optim.lr_scheduler.StepLR(opt, step_size=hp.opt_decay_step, gamma=hp.opt_decay_rate)
+    elif hp.opt_scheduler == "cos":
+        sched = torch.optim.lr_scheduler.CosineAnnealingLR(opt, T_max=hp.opt_restart)
+    return opt, sched
+
+
+def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0, hp=None, graph_mode=False, trace=None,
+                        bn=False):
+    """Port of Explainer.explain(..., unconstrained=True) (explain.py:97-146,209-211) with ExplainModule.{forward (unconstrained
+    branch), loss, mask_density} (explain.py:680-808) inlined.  Arguments as gnnx_oracle.explain_dense_torch; M0 (n,n) float32, every
+    entry of which is a parameter here.  trace: list receiving per epoch what print_training prints (loss, density, pred) and the terms.
+    mask_density keeps the CONSTRAINED _masked_adj (explain.py:680-683)."""
+    import torch
+    hp = hp or O.default_hparams()
+    W = weights if isinstance(weights, dict) and "conv_w" in weights else O.weights_to_torch(weights)
+    n = sub_adj.shape[0]
+    adj = torch.tensor(np.asarray(sub_adj)[None], dtype=torch.float)            # explain.py:97
+    x = torch.tensor(np.asarray(sub_feat)[None], requires_grad=True, dtype=torch.float)  # :98
+    mask = torch.nn.Parameter(torch.tensor(np.asarray(M0), dtype=torch.float))  # explain.py:646-652
+    feat_mask = torch.nn.Parameter(torch.zeros(x.size(-1)))                     # explain.py:633-643
+    diag_mask = torch.ones(n, n) - torch.eye(n)                                 # explain.py:617
+    opt, sched = _optimizer(hp, [mask, feat_mask])
+    params = [mask, feat_mask] + W["conv_w"] + [b for b in W["conv_b"] if b is not None] + [W["pred_w"], W["pred_b"]]
+    pred_label_t = None if graph_mode else torch.tensor(np.asarray(pred_label), dtype=torch.float)
+
+    def constrained_adj_fn():                                                   # explain.py:665-678 (mask_density only)
+        sym = torch.sigmoid(mask)
+        sym = (sym + sym.t()) / 2
+        return adj * sym * diag_mask
+
+    masked_adj = None
+    for epoch in range(hp.num_epochs):                                          # explain.py:137
+        for p in params:
+            p.grad = None
+        if x.grad is not None:
+            x.grad = None
+        sym = torch.sigmoid(mask)                                               # explain.py:688-692
+        masked_adj = torch.unsqueeze((sym + sym.t()) / 2, 0) * diag_mask
+        ypred = O._gcn_forward_torch(x, masked_adj, W, graph_mode, bn)          # explain.py:709, raw features
+        if graph_mode:
+            res = torch.softmax(ypred[0], dim=0)                                # explain.py:711
+        else:
+            res = torch.softmax(ypred[-1, node_idx_new, :], dim=0)              # explain.py:713-714
+        pred_loss = -torch.log(res[int(gt_label)])                              # explain.py:750-753
+        m = torch.sigmoid(mask)                                                 # explain.py:756-757
+        size_loss = hp.size * torch.sum(m)                                      # explain.py:760
+        fm = torch.sigmoid(feat_mask)
+        feat_size_loss = hp.feat_size * torch.mean(fm)                          # explain.py:766
+        mask_ent = -m * torch.log(m) - (1 - m) * torch.log(1 - m)               # explain.py:769
+        mask_ent_loss = hp.ent * torch.mean(mask_ent)                           # explain.py:770
+        if graph_mode:
+            lap_loss = 0                                                        # explain.py:787-788
+        else:
+            D = torch.diag(torch.sum(masked_adj[0], 0))                         # explain.py:780
+            Lm = D - masked_adj[-1]                                             # explain.py:781-782
+            lap_loss = hp.lap * (pred_label_t @ Lm @ pred_label_t) / adj.numel()  # explain.py:789-793
+        loss = pred_loss + size_loss + lap_loss + mask_ent_loss + feat_size_loss  # explain.py:808
+        loss.backward()                                                         # explain.py:142
+        opt.step()                                                              # explain.py:144
+        if sched is not None:
+            sched.step()                                                        # explain.py:145-146
+        with torch.no_grad():
+            density = torch.sum(constrained_adj_fn()) / torch.sum(adj)          # explain.py:148,680-683
+        if trace is not None:
+            v = lambda t: float(t.detach()) if torch.is_tensor(t) else float(t)
+            trace.append(dict(loss=v(loss), density=v(density), pred=res.detach().numpy().copy(), pred_loss=v(pred_loss),
+                              lap=v(lap_loss), feat_size=v(feat_size_loss), size=v(size_loss), ent=v(mask_ent_loss)))
+    return masked_adj[0].detach().numpy() * np.asarray(sub_adj, dtype=np.float64)   # explain.py:209-211
+
+
+def _lr_at(hp, t):
+    """Learning rate of update t (1-based) under the scheduler, stepped once per epoch after the optimiser (explain.py:144-146)."""
+    e = t - 1
+    if hp.opt_scheduler == "step":
+        return hp.lr * hp.opt_decay_rate ** (e // hp.opt_decay_step)
+    if hp.opt_scheduler == "cos":
+        return hp.lr * 0.5 * (1.0 + math.cos(math.pi * e / hp.opt_restart))
+    return hp.lr
+
+
+def _opt_update(hp, t, f, P, G, m_, v_):
+    """One in-place update of utils/train_utils.py:7-23's optimisers (torch defaults; SGD momentum 0.95) at update t."""
+    lr = _lr_at(hp, t)
+    if hp.opt == "adam":
+        b1t = 1 - hp.beta1 ** t; b2t = 1 - hp.beta2 ** t
+        m_ += (G - m_) * f(1 - hp.beta1)
+        v_ *= f(hp.beta2); v_ += f(1 - hp.beta2) * G * G
+        P -= f(lr / b1t) * m_ / (np.sqrt(v_) / f(math.sqrt(b2t)) + f(hp.eps))
+    elif hp.opt == "sgd":
+        m_ *= f(0.95); m_ += G
+        P -= f(lr) * m_
+    elif hp.opt == "rmsprop":
+        v_ *= f(0.99); v_ += f(0.01) * G * G
+        P -= f(lr) * G / (np.sqrt(v_) + f(1e-8))
+    elif hp.opt == "adagrad":
+        v_ += G * G
+        P -= f(lr) * G / (np.sqrt(v_) + f(1e-10))
+    else:
+        raise ValueError(hp.opt)
+
+
+def explain_closed_form(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0, hp=None, graph_mode=False, dtype=np.float64,
+                        return_state=False, bn=False):
+    """Hand-derived forward / backward of the unconstrained optimisation, any number of layers, --bn, every optimiser and scheduler.
+    The forward's adjacency is a = (1 - I) (.) (S + S^T)/2 with S = sigmoid(M) over all n^2 entries, the features are unmasked (so F is
+    moved by feat_size alone), the Laplacian term covers every pair (node mode).  return_state=True also returns M, F and the
+    one-step gradients gM, gF of the last update (with num_epochs=1: the gradients at M0, F = 0)."""
+    hp = hp or O.default_hparams()
+    f = dtype
+    X = np.asarray(sub_feat, dtype=f)
+    n, d = X.shape
+    A = 1 - np.eye(n, dtype=f)                                                     # diag_mask (explain.py:617,692)
+    Ws, bs = [], []
+    l = 1
+    while ("W%d" % l) in weights:
+        Ws.append(np.asarray(weights["W%d" % l], dtype=f))
+        b = weights.get("b%d" % l)
+        bs.append(np.zeros(Ws[-1].shape[1], f) if b is None else np.asarray(b, dtype=f))
+        l += 1
+    L = len(Ws)
+    dims = [w.shape[1] for w in Ws]
+    offs = np.concatenate([[0], np.cumsum(dims)])
+    Wp = np.asarray(weights["Wp"], dtype=f)
+    bp = np.asarray(weights["bp"], dtype=f)
+    r = int(node_idx_new)
+    M = np.asarray(M0, dtype=f).copy()
+    mM = np.zeros_like(M); vM = np.zeros_like(M)
+    F = np.zeros(d, f); mF = np.zeros(d, f); vF = np.zeros(d, f)
+    if not graph_mode:
+        y = np.asarray(pred_label, dtype=f)
+        lapA = (y[None, :] ** 2 - y[:, None] * y[None, :]) / f(n * n) * f(hp.lap)   # d/dA_ij of y^T(D-A)y/n^2
+    else:
+        lapA = np.zeros((n, n), f)
+    a = gM = gF = None
+    for t in range(1, hp.num_epochs + 1):
+        S = O._sigmoid(M)
+        a = A * (S + S.T) / 2                                                       # explain.py:688-692
+        if t == hp.num_epochs and not return_state:
+            break
+        sF = O._sigmoid(F)
+        H = [X]
+        Yh, q, bn_state = [], [], []
+        for l in range(L):
+            Y = (a @ H[-1]) @ Ws[l] + bs[l]                                         # models.py:70-76
+            ql = np.maximum(np.sqrt((Y * Y).sum(1, keepdims=True)), f(1e-12))       # F.normalize eps
+            Yl = Y / ql
+            Yh.append(Yl); q.append(ql)
+            if l < L - 1:
+                Hl = np.maximum(Yl, 0)
+                if bn:                                                                 # BatchNorm1d(n), train mode, no affine
+                    mu = Hl.mean(1, keepdims=True)
+                    istd = 1 / np.sqrt(((Hl - mu) ** 2).mean(1, keepdims=True) + f(1e-5))
+                    Hl = (Hl - mu) * istd
+                    bn_state.append((Hl, istd))
+                H.append(Hl)
+            else:
+                H.append(Yl)
+        dE = [np.zeros((n, dims[l]), f) for l in range(L)]
+        if graph_mode:
+            pooled = [H[l + 1].max(0) for l in range(L)]
+            arg = [H[l + 1].argmax(0) for l in range(L)]          # first max index, like torch.max
+            emb = np.concatenate(pooled)
+        else:
+            emb = np.concatenate([H[l + 1][r] for l in range(L)])
+        logits = Wp @ emb + bp
+        p = np.exp(logits - logits.max()); p = p / p.sum()
+        g = p.copy(); g[int(gt_label)] -= 1                                          # d(-log p[gt])/dlogits
+        dEmb = Wp.T @ g
+        for l in range(L):
+            sl = dEmb[offs[l]:offs[l + 1]]
+            if graph_mode:
+                dE[l][arg[l], np.arange(dims[l])] += sl
+            else:
+                dE[l][r] += sl
+        dA = lapA.copy()
+        dH = np.zeros((n, dims[L - 1]), f)
+        for l in range(L - 1, -1, -1):
+            dYh = dE[l] + dH
+            if l < L - 1:
+                if bn:                                                                 # backward of the row standardisation
+                    Hb, istd = bn_state[l]
+                    dYh = (dYh - dYh.mean(1, keepdims=True) - Hb * (dYh * Hb).mean(1, keepdims=True)) * istd
+                dYh = dYh * (Yh[l] > 0)
+            dY = (dYh - Yh[l] * (Yh[l] * dYh).sum(1, keepdims=True)) / q[l]          # backward of x/max(|x|,eps)
+            dZ = dY @ Ws[l].T
+            dA += dZ @ H[l].T
+            dH = a.T @ dZ
+        gF = sF * (1 - sF) * (f(hp.feat_size) / f(d))                                # the forward never sees F
+        # size = c*sum(S), ent = mean(H(S)) over ALL n^2 entries; the diagonal gets the regularisers only (A_ii = 0)
+        gM = S * (1 - S) * ((A * dA + (A * dA).T) / 2 + f(hp.size) - f(hp.ent) * M / f(n * n))
+        for P, G, m_, v_ in ((M, gM, mM, vM), (F, gF, mF, vF)):
+            _opt_update(hp, t, f, P, G, m_, v_)
+    out = a.astype(np.float64) * np.asarray(sub_adj, dtype=np.float64)
+    if return_state:
+        return out, dict(M=M, F=F, gM=gM, gF=gF)
+    return out

@@ -2,7 +2,7 @@
 """Small invocation of every kernel for compute-sanitizer (racecheck / memcheck / synccheck are ~100x slower than a plain run):
     compute-sanitizer --tool racecheck python tools/sanitize_run.py
 k-hop extraction + shared-memory kernel on a mix of task sizes (syn1: hub node 0 and tiny tasks), the streaming kernel (forced),
-the gradient baseline, graph mode, densify, neighbourhood rows.  A few epochs each."""
+the gradient baseline, graph mode, densify, neighbourhood rows, the unconstrained (dense) kernel.  A few epochs each."""
 import os
 import sys
 
@@ -19,7 +19,7 @@ EPOCHS = int(os.environ.get("SAN_EPOCHS", "4"))
 
 
 def main():
-    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster"]
+    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster", "dense"]
     fx = util.load_fixture("syn1")
     if "node" in which:
         eng = util.make_engine(fx)
@@ -95,6 +95,41 @@ def main():
         out = np.zeros(int(eoff[-1]), np.float32)
         eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS), m0, out)
         print("graph ok", float(out.sum()))
+        eng.close()
+    if "dense" in which:   # explain_dense.cu: node mode with a trace, a --bn 4-layer model with SGD, graph mode
+        import gnnx_oracle as O
+        eng = util.make_engine(fx)
+        plan = eng.plan_nodes([300, 5, 13], 3)
+        n_t = [plan.n(t) for t in range(plan.count)]
+        m0 = np.concatenate([O.draw_m0(n, seed=n).reshape(-1) for n in n_t])
+        out = np.zeros(plan.total_edges, np.float32)
+        md = np.zeros(sum(n * n for n in n_t), np.float32)
+        tr = np.zeros((plan.count, EPOCHS, _abi.GX_TRACE_COLS), np.float32)
+        tp = np.zeros((plan.count, EPOCHS, eng.num_classes), np.float32)
+        eng.explain_nodes_unconstrained(eng.make_hparams(num_epochs=EPOCHS), m0, out, md, tr, tp)
+        print("dense ok node", float(out.sum()), float(tr.sum()))
+        eng.close()
+        rng = np.random.default_rng(6)
+        sc = lambda *s_: (rng.normal(size=s_) * 0.4).astype(np.float32)
+        d0 = fx.feat.shape[1]
+        C0 = fx.weights["Wp"].shape[0]
+        w4 = dict(W1=sc(d0, 40), b1=sc(40), W2=sc(40, 40), b2=sc(40), W3=sc(40, 40), b3=sc(40), W4=sc(40, 24), b4=sc(24), Wp=sc(C0, 144), bp=sc(C0))
+        eng = gnnx.Engine(0)
+        eng.set_model(w4, num_layers=4, bn=True)
+        eng.set_graph_csr(fx.rowptr, fx.col, fx.feat, fx.label, fx.pred_label)
+        plan = eng.plan_nodes([300, 5], 4)
+        out = np.zeros(plan.total_edges, np.float32)
+        eng.explain_nodes_unconstrained(eng.make_hparams(num_epochs=EPOCHS, opt=1, init=_abi.GX_INIT_PHILOX, seed=4), None, out)
+        print("dense ok bn L4 sgd", float(out.sum()))
+        eng.close()
+        g = np.load(util.GOLDEN + "/graphs_golden.npz")
+        eng = gnnx.Engine(0)
+        eng.set_model({k: g[k] for k in util.WKEYS})
+        eng.set_graph_batch(g["adj"], g["feat"], g["label"])
+        eoff = eng.plan_graphs([0, 3, 5])
+        out = np.zeros(int(eoff[-1]), np.float32)
+        eng.explain_graphs_unconstrained(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=5), None, out)
+        print("dense ok graph", float(out.sum()))
         eng.close()
     if "misc" in which:
         eng = util.make_engine(fx)
