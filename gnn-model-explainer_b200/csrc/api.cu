@@ -11,6 +11,7 @@
 #include <cmath>
 #include <iterator>
 #include <memory>
+#include <numeric>
 #include <vector>
 
 #include "host.cuh"
@@ -201,6 +202,28 @@ int place_pair_slabs(gx_handle* h, GxExplainLaunch* cfg, const int* slabs, int n
   return GX_OK;
 }
 
+int launch_var_batch(gx_handle* h, const char* who, int graph_mode, const GxHparamsDev& hd, const IoDev& D) {
+  const int bytes = gx_var_smem_bytes(graph_mode, h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C);
+  if (bytes > gx_explain_max_smem()) { gx_set_error("%s: model does not fit the variant kernel", who); return GX_ERR_UNSUPPORTED; }
+  int max_ctas = h->num_sms * 4;
+  if (graph_mode) {   // graph mode: as many CTAs as are co-resident
+    const int per_sm = gx_var_ctas_per_sm(graph_mode, h->m);
+    if (per_sm < 1) { gx_set_error("%s: the variant kernel cannot be resident (%d bytes of shared memory)", who, bytes); return GX_ERR_UNSUPPORTED; }
+    max_ctas = h->num_sms * per_sm;
+  }
+  std::vector<int32_t> all(h->count);
+  std::iota(all.begin(), all.end(), 0);
+  GxExplainLaunch cfg{};
+  cfg.order = h->d_order.as<int32_t>(); cfg.ntasks = h->count; cfg.counter = h->d_counters.as<int32_t>(); cfg.x = D.x;
+  int rc = size_slab_launch(h, who, all, [&](const GxTask& T) { return var_slab_words(h, graph_mode, T); }, max_ctas, &cfg);
+  if (rc == GX_OK) rc = place_pair_slabs(h, &cfg, &cfg.grid, 1);
+  if (rc == GX_OK) rc = begin_timing(h);
+  if (rc != GX_OK) return rc;
+  GX_CUDA_CHECK(gx_launch_explain_var(cfg, graph_mode, h->g, h->gb, h->m, hd, h->plan, D.m0, D.out, D.feat, h->stream));
+  h->launches += 1;
+  return GX_OK;
+}
+
 extern "C" {
 
 const char* gx_last_error(void) { return g_err; }
@@ -377,7 +400,7 @@ int gx_set_model(gx_handle* h, const gx_model_dims* dims, const float* const* co
   if (dims->num_layers != 3 || (dims->flags & GX_MODEL_BN) || dims->hidden_dim > 32 || dims->embed_dim > 32) {
     // Model variant (num_gc_layers 2 / 4, --bn, widths 33..128): explain_var.cu, true widths (a zero-padded column would enter the bn statistics).
     const int L = dims->num_layers, d = dims->input_dim, hid0 = dims->hidden_dim, emb0 = dims->embed_dim, C = dims->num_classes;
-    if (gx_var_smem_bytes(d, L, hid0, emb0, C) > gx_explain_max_smem()) { gx_set_error("gx_set_model: model variant does not fit shared memory"); return GX_ERR_UNSUPPORTED; }
+    if (gx_var_smem_bytes(0, d, L, hid0, emb0, C) > gx_explain_max_smem()) { gx_set_error("gx_set_model: model variant does not fit shared memory"); return GX_ERR_UNSUPPORTED; }
     std::vector<float> host;
     size_t offW[GX_MAX_LAYERS], offb[GX_MAX_LAYERS];
     auto al4 = [&]() { while (host.size() % 4) host.push_back(0.f); };

@@ -146,12 +146,8 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
   float* const slab = A.gws + (int64_t)blockIdx.x * A.gws_stride_words;
 
   for (;;) {
-    __syncthreads();
-    if (tid == 0) s_task = atomicAdd(A.counter, 1);
-    __syncthreads();
-    const int qi = s_task;
-    if (qi >= A.ntasks) break;
-    const int task_id = A.order[qi];
+    int task_id;
+    if (!var_next_task(A, s_task, tid, task_id)) break;
     const GxTask* __restrict__ Tp = A.plan.tasks + task_id;
     const int n = graph ? A.gb.max_nodes : Tp->n;
     const int r = graph ? 0 : Tp->idx_new;
@@ -164,6 +160,7 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
     float* const Hc = slab + Lo.Hc; float* const dZc = slab + Lo.dZc; float* const Z = slab + Lo.Z;
     auto off = [&](int l) { return l == 0 ? 0 : Lo.off1 + (l - 1) * VW; };   // column of H_l (and of dZ_{l+1}) in Hc / dZc
     auto Yh = [&](int l) { return slab + Lo.Yh + (int64_t)(l - 1) * n * VW; };
+    auto Hl = [&](int l) { return Hc + off(l); };
     auto qn = [&](int l) { return slab + Lo.q + (int64_t)(l - 1) * n; };
     auto istd = [&](int l) { return slab + Lo.istd + (int64_t)(l - 1) * n; };
     // this task's rows: canonical (ascending-id) k-hop set in node mode, the padded graph in graph mode
@@ -224,35 +221,13 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
         const float* const Ws = Wl[l - 1]; const float* const bsm = sm + S.b[l - 1];
         for (int i = warp; i < n; i += nwarps) {
           for (int f = lane; f < win; f += 32) zs[f] = Z[(int64_t)i * ZW + f];
-          __syncwarp();
-          float y[KW];
-          var_dense<KW>(zs, win, Ws, wout, bsm, y, lane);
-          __syncwarp();
-          float yh[KW], h[KW], is = 1.f;
-          const float q = var_activate<kBn, KW>(y, wout, l < L, yh, h, &is, lane);
-          if (kBn && l < L && lane == 0) istd(l)[i] = is;
-#pragma unroll
-          for (int k = 0; k < KW; ++k) {
-            Yh(l)[(int64_t)i * VW + lane + 32 * k] = yh[k];
-            Hc[(int64_t)i * KH + off(l) + lane + 32 * k] = lane + 32 * k < wout ? h[k] : 0.f;
-          }
-          if (lane == 0) qn(l)[i] = q;
+          var_row_forward<kBn, KW>(zs, win, Ws, wout, bsm, l, L, i, Yh, Hl, KH, qn, istd, lane);
         }
         __syncthreads();
       }
       // ---------------------------------------------------------------- S: readout, softmax, dEmb   (explain.py:709-714)
       if (graph) {
-        for (int k = tid; k < PD; k += NT) {   // per-layer max-pool over all padded rows (models.py:283,291,300), first maximum wins
-          const int l = k < hid * (L - 1) ? k / hid + 1 : L;
-          const int c = k - hid * (l - 1);
-          float best = -INFINITY;
-          int bi = 0;
-          for (int i = 0; i < n; ++i) {
-            const float v = Hc[(int64_t)i * KH + off(l) + c];
-            if (v > best) { best = v; bi = i; }
-          }
-          emb[k] = best; arg[k] = bi;
-        }
+        var_max_pool(L, hid, PD, n, Hl, KH, nullptr, 0, emb, arg, tid, NT);   // over all padded rows
       } else if (warp == 0) {
         for (int l = 1; l <= L; ++l)
           for (int c = lane; c < wout_of(l - 1); c += 32) emb[hid * (l - 1) + c] = Hc[(int64_t)r * KH + off(l) + c];
@@ -284,12 +259,7 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
             if (c < wout && (graph ? arg[koff + c] == i : i == r)) g[k] += dEmb[koff + c];
             yh[k] = Yh(l)[(int64_t)i * VW + c];
           }
-          if (l < L) var_hidden_backward<kBn, KW>(g, yh, Hc + (int64_t)i * KH + off(l), kBn ? istd(l)[i] : 1.f, wout, lane);
-          const float sdot = var_norm_dot<KW>(g, yh, wout, lane);
-          const float qi = qn(l)[i];
-          __syncwarp();
-          var_norm_backward<KW>(g, yh, sdot, qi, wout, zs, lane);   // dY: backward of y / max(|y|, eps)
-          __syncwarp();
+          var_row_backward<kBn, KW>(g, yh, l, L, i, Hl, KH, qn, istd, wout, zs, lane);
           if (l == 1) {   // dZ_1 = dY W_1^T, width d (the features are not masked: no dL/dsF)
             for (int f = lane; f < d; f += 32) {
               float t = 0.f;
@@ -376,20 +346,6 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
   }
 }
 
-// calls f(kernel) with the instantiation for the model
-template <typename F>
-cudaError_t with_dense_kernel(const GxModelDev& m, F&& f) {
-  const int kw = var_kw(m.hid, m.emb);
-  if (m.bn) {
-    if (kw == 1) return f(explain_dense_kernel<true, 1>);
-    if (kw == 2) return f(explain_dense_kernel<true, 2>);
-    return f(explain_dense_kernel<true, 4>);
-  }
-  if (kw == 1) return f(explain_dense_kernel<false, 1>);
-  if (kw == 2) return f(explain_dense_kernel<false, 2>);
-  return f(explain_dense_kernel<false, 4>);
-}
-
 }  // namespace
 
 int gx_dense_smem_bytes(int d, int L, int hid, int emb, int C) { return dense_smem(d, L, hid, emb, C, kVarThreads / 32).total * 4; }
@@ -398,14 +354,8 @@ int gx_dense_smem_bytes(int d, int L, int hid, int emb, int C) { return dense_sm
 int gx_dense_ctas_per_sm(const GxModelDev& m) {
   const int bytes = gx_dense_smem_bytes(m.d, m.L, m.hid, m.emb, m.C);
   int n = 0;
-  const cudaError_t e = with_dense_kernel(m, [&](auto kern) -> cudaError_t {
-    cudaError_t r = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (r != cudaSuccess) return r;
-    r = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (r != cudaSuccess) return r;
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, kVarThreads, bytes);
-  });
-  return e == cudaSuccess ? n : 0;
+  var_dispatch(m, [&](auto bn, auto kw) { n = var_ctas_per_sm(explain_dense_kernel<decltype(bn)::value, decltype(kw)::value>, bytes); return cudaSuccess; });
+  return n;
 }
 
 cudaError_t gx_launch_explain_dense(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
@@ -416,12 +366,7 @@ cudaError_t gx_launch_explain_dense(const GxExplainLaunch& cfg, int graph_mode, 
   args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
   args.graph_mode = graph_mode; args.g = g; args.gb = gb; args.m = m; args.hp = hp; args.plan = plan; args.io = io;
   const int bytes = gx_dense_smem_bytes(m.d, m.L, m.hid, m.emb, m.C);
-  return with_dense_kernel(m, [&](auto kern) -> cudaError_t {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e != cudaSuccess) return e;
-    kern<<<cfg.grid, kVarThreads, bytes, s>>>(args);
-    return cudaGetLastError();
+  return var_dispatch(m, [&](auto bn, auto kw) {
+    return var_launch(explain_dense_kernel<decltype(bn)::value, decltype(kw)::value>, args, cfg.grid, bytes, s);
   });
 }

@@ -1,19 +1,50 @@
-// explain_var.cu -- K2v: the mask-optimisation kernel for the model VARIANTS of the reference (SURVEY 8 row f3):
+// explain_var.cu -- K2v: the mask-optimisation kernel for the model and optimiser VARIANTS of the reference (SURVEY 8 row f3), node
+// mode and graph-classification mode:
 //   num_gc_layers = 2 / 3 / 4 (explainer_main.py:57-66, explain.py:64: n_hops = num_gc_layers; models.py:193-220,230-267) and
 //   --bn (models.py:222-228: a FRESH BatchNorm1d(n) in train mode on the (1, n, h) activations = per-node standardisation over
 //   the feature axis, eps 1e-5, biased variance, applied after the ReLU of every hidden layer; the readout concatenates the
-//   standardised activations, models.py:241-260).
-// It computes exactly what oracle/kernel_spec.py specifies (parameters on the directed edges, layer l only on the rows within
-// L - l hops of the explained node, inner / outer pair split), for hidden / output widths up to 128 (the tuned kernels stop at 32) and d <= 128.  These options are rare, so the
-// kernel is written for clarity, not speed: one persistent CTA per task, state in a per-CTA global slab (L2 resident for the
-// reference's graph sizes), one warp per row with lane = feature, one thread per undirected edge in the edge phase.
-// Phases per epoch (one __syncthreads each): F1 .. FL | S | BL .. B1 | P.  The default model (3 layers, no bn) never comes here.
+//   standardised activations, models.py:241-260), hidden / output widths up to 128 (the tuned kernels stop at 32), d <= 128, and
+//   the optimisers of utils/train_utils.py:7-23 (Adam, SGD momentum 0.95, RMSprop, Adagrad; step / cos schedulers).
+// Node mode computes exactly what oracle/kernel_spec.py specifies (parameters on the directed edges, layer l only on the rows within
+// L - l hops of the explained node, inner / outer pair split) and reads out row 0 (the explained node in level order).
+// Graph mode replaces Explainer.explain(node_idx=0, graph_idx=g, graph_mode=True) (explain.py:80-85,137-146,209-211; loss :740-808
+// with lap_loss = 0) on a GcnEncoderGraph (models.py:269-316), as explain_graph.cu generalised to L layers:
+//   * no receptive-field pruning: every row with at least one edge is computed at every layer; rows WITHOUT an edge (padding,
+//     isolated nodes) all hold one per-layer constant, bn(relu(normalize(b_l))) / normalize(b_L), independent of the masks -- it joins
+//     every max-pool and never carries gradient to M or F;
+//   * readout = per-layer column max over the padded rows (the constant first, then the rows in ascending order; the first maximum
+//     takes the gradient), concatenation, Linear, softmax, -log p[graph label];
+//   * every edge gets SDDMM terms from all L layers; the 1/n^2 of the entropy term and the std of M0 use the PADDED size.
+// These options are rare, so the kernel is written for clarity, not speed: one persistent CTA per task, state in a per-CTA global slab
+// (GxVarLayout, L2 resident for the reference's graph sizes), one warp per row with lane = feature, one thread per undirected edge in
+// the edge phase.  Phases per epoch (one __syncthreads each): F1 .. FL | (graph mode: pool) | S | BL .. B1 | P.  The default model
+// (3 layers, no bn) with Adam never comes here.
 #include "explain_var_common.cuh"
 
 namespace {
 
-template <bool kBn, int KW>
-__global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainArgs A) {
+struct VarArgs {
+  const int32_t* order;
+  int32_t ntasks;
+  int32_t* counter;
+  float* gws;
+  int64_t gws_stride_words;
+  float* pws;
+  int64_t pws_stride_words;
+  GxGraphDev g;          // node mode
+  GxGraphBatchDev gb;    // graph mode
+  GxModelDev m;
+  GxHparamsDev hp;
+  GxPlanArrays plan;
+  const float* m0;
+  float* out_mask;
+  float* out_feat;
+};
+
+// The minimum-blocks bound 0 is the compiler's default: node mode is capped at 128 registers (some instantiations spill); graph mode
+// lets the small default-width model fit two CTAs per SM.
+template <bool kGraph, bool kBn, int KW>
+__global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1) : 0) explain_var_kernel(const VarArgs A) {
   extern __shared__ __align__(16) float sm[];
   __shared__ int s_task;
   constexpr int NT = kVarThreads, nwarps = NT / 32;
@@ -30,6 +61,8 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
   float* const zs = sm + S.zs + warp * S.zlen;
   float* const gFp = sm + S.gFp;
   float* const emb = sm + S.emb; float* const dEmb = sm + S.dEmb; float* const logit = sm + S.logit;
+  float* const cst = sm + S.total;                                              // graph mode (gx_var_smem_bytes)
+  int* const arg = reinterpret_cast<int*>(sm + S.total + gx_round_up(PD, 4));   // graph mode
   const bool wp_smem = C * (PD + 1) <= GX_WP_SMEM_MAX;
   const float* const Wpp = wp_smem ? sm + S.Wp : m.Wp;
   const float* const bpp = wp_smem ? sm + S.Wp + C * PD : m.bp;
@@ -38,24 +71,41 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
 
   const float* Wl[GX_MAX_LAYERS];   // conv weights: shared memory when they fit, else global (L2 resident)
   var_stage_model(m, S, sm, Wl, tid, NT);
+  if constexpr (kGraph) {
+    __syncthreads();
+    // embedding of a row without edges: Y = 0 W + b, the same activation as any row; depends on the model only
+    if (warp == 0) {
+      for (int l = 1; l <= L; ++l) {
+        const int wout = wout_of(l - 1);
+        float y[KW], yh[KW], h[KW], is;
+        var_dense<KW>(zs, 0, Wl[l - 1], wout, sm + S.b[l - 1], y, lane);
+        var_activate<kBn, KW>(y, wout, l < L, yh, h, &is, lane);
+#pragma unroll
+        for (int k = 0; k < KW; ++k)
+          if (lane + 32 * k < wout) cst[hid * (l - 1) + lane + 32 * k] = h[k];
+      }
+    }
+  }
   float* const slab = A.gws + (int64_t)blockIdx.x * A.gws_stride_words;
-  float2* const MM0 = reinterpret_cast<float2*>(A.pws + (int64_t)blockIdx.x * A.pws_stride_words);
+  float2* const MM = reinterpret_cast<float2*>(A.pws + (int64_t)blockIdx.x * A.pws_stride_words);
 
   for (;;) {
-    __syncthreads();
-    if (tid == 0) s_task = atomicAdd(A.counter, 1);
-    __syncthreads();
-    const int qi = s_task;
-    if (qi >= A.ntasks) break;
-    const int task_id = A.order[qi];
+    int task_id;
+    if (!var_next_task(A, s_task, tid, task_id)) break;
     const GxTask* __restrict__ Tp = A.plan.tasks + task_id;
-    const int n = Tp->n, n2 = Tp->n2, e1 = Tp->e1, np = Tp->npairs_in;
+    // graph mode: n = the rows with an edge, n2 = n, e1 = e_d, npairs_in = npairs (gx_plan_graphs)
+    const int n = Tp->n, n2 = kGraph ? n : Tp->n2, e1 = Tp->e1, np = Tp->npairs_in;
     const int gt = Tp->gt_label;
     const int64_t node_off = Tp->node_off, rp_off = Tp->rp_off, edge_off = Tp->edge_off, pair_off = Tp->pair_off;
-    int R[GX_MAX_LAYERS + 1];   // R[l] = rows of layer l (1-based): nodes within L - l hops; R[0] = n
-    R[0] = n;
-    for (int l = 1; l <= L; ++l) R[l] = Tp->cum[L - l] < n ? Tp->cum[L - l] : n;
-    const GxVarLayout Lo = gx_make_var_layout(n, n2, e1, np, d, L, VW);
+    int R[GX_MAX_LAYERS + 1];   // node mode: R[l] = rows of layer l (1-based): nodes within L - l hops; R[0] = n
+    if constexpr (!kGraph) {
+      R[0] = n;
+      for (int l = 1; l <= L; ++l) R[l] = Tp->cum[L - l] < n ? Tp->cum[L - l] : n;
+    }
+    auto rows = [&](int l) { if constexpr (kGraph) return n; else return R[l]; };
+    const GxVarLayout Lo = gx_make_var_layout(n, n2, e1, kGraph ? 0 : np, d, L, VW);
+    // layer 1's input rows: the graph's features (node mode), this graph's padded rows (graph mode); both indexed by lo2gid
+    const float* const feat = kGraph ? A.gb.feat + (int64_t)Tp->node * A.gb.max_nodes * d : A.g.feat;
     const int32_t* __restrict__ lo2gid = A.plan.lo2gid + node_off;
     const int32_t* __restrict__ irp = A.plan.irowptr + rp_off;
     const int32_t* __restrict__ icol = A.plan.icol + edge_off;
@@ -68,8 +118,8 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
     auto dZ = [&](int l) { return slab + Lo.dZ + (int64_t)(l - 2) * n2 * VW; };     // l = 2..L: dL/d(A_m H_{l-1}) (width hid)
     auto qn = [&](int l) { return slab + Lo.q + (int64_t)(l - 1) * n2; };
     auto istd = [&](int l) { return slab + Lo.istd + (int64_t)(l - 1) * n2; };
-    float2* const MM = MM0; float2* const mm = MM + np; float2* const vv = mm + np; float2* const SS = vv + np;
-    const float nn = (float)n * (float)n;
+    float2* const mm = MM + np; float2* const vv = mm + np; float2* const SS = vv + np;
+    const float nn = (float)Tp->n_norm * (float)Tp->n_norm;
     const float ent_over_nn = hp.c_ent / nn;
     const float lap_over_nn = hp.c_lap / nn;
 
@@ -78,7 +128,7 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
       if (hp.out_iter == 0 && f < d && A.out_feat != nullptr) A.out_feat[(int64_t)task_id * d + f] = 0.5f;
     }
     {
-      const float m0_std = sqrtf(2.0f / (float)n);  // gain('relu') * sqrt(2/(n+n)) (explain.py:647-651)
+      const float m0_std = sqrtf(2.0f / (float)Tp->n_norm);  // gain('relu') * sqrt(2/(n+n)) (explain.py:647-651), n = the padded size in graph mode
       for (int p = tid; p < np; p += NT) {
         const int oij = poij[p], oji = poji[p];
         const float Mi = var_init_param(hp, A.m0, edge_off + oij, (uint32_t)Tp->node, (uint32_t)oij, m0_std);
@@ -90,10 +140,12 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
         SS[p] = make_float2(Si, Sj);
         const float a0 = 0.5f * (Si + Sj);  // explain.py:665-678
         const int i = pi[p], j = pj[p];
-        if (i < n2) a[ppij[p]] = a0;
-        if (j < n2) a[ppji[p]] = a0;
-        const float yd = (float)__ldg(A.g.pred_label + lo2gid[i]) - (float)__ldg(A.g.pred_label + lo2gid[j]);
-        lapg[p] = lap_over_nn * yd * yd;   // d/dA_ij + d/dA_ji of y^T (D - A) y / n^2 (explain.py:780-793)
+        if (kGraph || i < n2) a[ppij[p]] = a0;
+        if (kGraph || j < n2) a[ppji[p]] = a0;
+        if constexpr (!kGraph) {   // no Laplacian term in graph mode (explain.py:787-788)
+          const float yd = (float)__ldg(A.g.pred_label + lo2gid[i]) - (float)__ldg(A.g.pred_label + lo2gid[j]);
+          lapg[p] = lap_over_nn * yd * yd;   // d/dA_ij + d/dA_ji of y^T (D - A) y / n^2 (explain.py:780-793)
+        }
         if (hp.out_iter == 0) { A.out_mask[edge_off + oij] = a0; A.out_mask[edge_off + oji] = a0; }
       }
     }
@@ -104,31 +156,25 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
       for (int l = 1; l <= L; ++l) {
         const int win = win_of(l - 1), wout = wout_of(l - 1);
         const float* const Ws = Wl[l - 1]; const float* const bsm = sm + S.b[l - 1];
-        for (int i = warp; i < R[l]; i += nwarps) {
+        for (int i = warp; i < rows(l); i += nwarps) {
           const int r0 = irp[i], r1 = irp[i + 1];
-          if (l == 1) var_gather_feat(r0, r1, icol, a, A.g.feat, lo2gid, d, sF, U + (int64_t)i * dp, zs, lane);
+          if (l == 1) var_gather_feat(r0, r1, icol, a, feat, lo2gid, d, sF, U + (int64_t)i * dp, zs, lane);
           else var_gather_hidden<KW>(r0, r1, icol, a, Hh(l - 1), win, zs, lane);
-          __syncwarp();
-          float y[KW];
-          var_dense<KW>(zs, win, Ws, wout, bsm, y, lane);
-          __syncwarp();
-          float yh[KW], h[KW], is = 1.f;
-          const float q = var_activate<kBn, KW>(y, wout, l < L, yh, h, &is, lane);
-          if (kBn && l < L && lane == 0) istd(l)[i] = is;
-#pragma unroll
-          for (int k = 0; k < KW; ++k) {
-            Yh(l)[(int64_t)i * VW + lane + 32 * k] = yh[k];
-            Hh(l)[(int64_t)i * VW + lane + 32 * k] = lane + 32 * k < wout ? h[k] : 0.f;
-          }
-          if (lane == 0) qn(l)[i] = q;
+          var_row_forward<kBn, KW>(zs, win, Ws, wout, bsm, l, L, i, Yh, Hh, VW, qn, istd, lane);
         }
         __syncthreads();
       }
-      // ---------------------------------------------------------------- S: readout of row r = level-order id 0, softmax, dEmb
+      // ---------------------------------------------------------------- S: readout, softmax, dEmb   (models.py:305-314, explain.py:711)
+      if constexpr (kGraph) {   // max-pool of every layer, the edge-less rows' constant first
+        var_max_pool(L, hid, PD, n, Hh, VW, (Tp->flags & 1) != 0 ? cst : nullptr, -1, emb, arg, tid, NT);
+        __syncthreads();
+      }
       if (warp == 0) {
-        for (int l = 1; l <= L; ++l)
-          for (int c = lane; c < wout_of(l - 1); c += 32) emb[hid * (l - 1) + c] = Hh(l)[c];
-        __syncwarp();
+        if constexpr (!kGraph) {   // node mode reads out row r = level-order id 0
+          for (int l = 1; l <= L; ++l)
+            for (int c = lane; c < wout_of(l - 1); c += 32) emb[hid * (l - 1) + c] = Hh(l)[c];
+          __syncwarp();
+        }
         var_readout_tail(emb, Wpp, bpp, C, PD, gt, logit, dEmb, lane);
       }
       for (int idx = tid; idx < nwarps * dp; idx += NT) gFp[idx] = 0.f;
@@ -137,23 +183,20 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
       for (int l = L; l >= 1; --l) {
         const int win = win_of(l - 1), wout = wout_of(l - 1);
         const float* const Ws = Wl[l - 1];
-        for (int i = warp; i < R[l]; i += nwarps) {
+        const int koff = hid * (l - 1);
+        for (int i = warp; i < rows(l); i += nwarps) {
           // dL/dH_l[i] = (A_m^T dZ_{l+1})[i] over the neighbours that are rows of layer l+1 (a prefix of row i) + the readout's share
           float g[KW], yh[KW];
 #pragma unroll
           for (int k = 0; k < KW; ++k) g[k] = 0.f;
-          if (l < L) var_gather_back<KW>(irp[i], irp[i + 1], icol, a, dZ(l + 1), wout, R[l + 1], g, lane);   // columns are partitioned by level
+          if (l < L) var_gather_back<KW>(irp[i], irp[i + 1], icol, a, dZ(l + 1), wout, rows(l + 1), g, lane);   // columns are partitioned by level
 #pragma unroll
           for (int k = 0; k < KW; ++k) {
-            if (i == 0 && lane + 32 * k < wout) g[k] += dEmb[hid * (l - 1) + lane + 32 * k];
-            yh[k] = Yh(l)[(int64_t)i * VW + lane + 32 * k];
+            const int c = lane + 32 * k;
+            if (c < wout && (kGraph ? arg[koff + c] == i : i == 0)) g[k] += dEmb[koff + c];
+            yh[k] = Yh(l)[(int64_t)i * VW + c];
           }
-          if (l < L) var_hidden_backward<kBn, KW>(g, yh, Hh(l) + (int64_t)i * VW, kBn ? istd(l)[i] : 1.f, wout, lane);
-          const float sdot = var_norm_dot<KW>(g, yh, wout, lane);
-          const float qi = qn(l)[i];
-          __syncwarp();
-          var_norm_backward<KW>(g, yh, sdot, qi, wout, zs, lane);   // dY: backward of y / max(|y|, eps)
-          __syncwarp();
+          var_row_backward<kBn, KW>(g, yh, l, L, i, Hh, VW, qn, istd, wout, zs, lane);
           // dZ[f] = sum_c dY[c] W[f][c]
           if (l == 1) var_first_layer_dz(zs, Ws, d, wout, U + (int64_t)i * dp, sF, gFp + warp * dp, dZ1 + (int64_t)i * dp, lane);
           else var_hidden_dz<KW>(zs, Ws, win, wout, dZ(l) + (int64_t)i * VW, lane);
@@ -161,11 +204,11 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
         }
         __syncthreads();
       }
-      // ---------------------------------------------------------------- P: edge gradients, regularisers, Adam, next mask
+      // ---------------------------------------------------------------- P: edge gradients, regularisers, optimiser step, next mask
       {
         const float2 tab = __ldg(hp.adam_tab + (it - 1));
         const float step = tab.x, bc2s = tab.y, bc2s_inv = 1.0f / tab.y;
-        const bool last = (it == hp.out_iter);
+        const bool last = (it == hp.out_iter);   // the mask built after this update is the one the reference returns
         for (int f = tid; f < d; f += NT) {
           float gsum = 0.f;
           for (int w = 0; w < nwarps; ++w) gsum += gFp[w * dp + f];
@@ -180,23 +223,43 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
         }
         for (int p = tid; p < np; p += NT) {
           const int i = pi[p], j = pj[p];   // i < j in level order
-          float Gd = lapg[p];
-          if (i < R[1]) {
-            float t = 0.f;
-            const float* xr = A.g.feat + (int64_t)lo2gid[j] * d;
-            for (int f = 0; f < d; ++f) t = fmaf(dZ1[(int64_t)i * dp + f], __ldg(xr + f), t);
-            Gd += t;
-          }
-          if (j < R[1]) {
-            float t = 0.f;
-            const float* xr = A.g.feat + (int64_t)lo2gid[i] * d;
-            for (int f = 0; f < d; ++f) t = fmaf(dZ1[(int64_t)j * dp + f], __ldg(xr + f), t);
-            Gd += t;
-          }
-          for (int l = 2; l <= L; ++l) {
-            const float* const dZl = dZ(l); const float* const Hp = Hh(l - 1);
-            if (i < R[l]) { float t = 0.f; for (int f = 0; f < hid; ++f) t = fmaf(dZl[(int64_t)i * VW + f], Hp[(int64_t)j * VW + f], t); Gd += t; }
-            if (j < R[l]) { float t = 0.f; for (int f = 0; f < hid; ++f) t = fmaf(dZl[(int64_t)j * VW + f], Hp[(int64_t)i * VW + f], t); Gd += t; }
+          // dL/dA_ij + dL/dA_ji = sum over the layers of <dL/d(A_m H_{l-1})[i], H_{l-1}[j]> + <.. [j], .. [i]> (layer 1: feature rows)
+          float Gd;
+          if constexpr (kGraph) {   // no Laplacian term; every row at every layer, both directions of a layer in one sum
+            Gd = 0.f;
+            {
+              const float* xi = feat + (int64_t)lo2gid[i] * d; const float* xj = feat + (int64_t)lo2gid[j] * d;
+              float t = 0.f;
+              for (int f = 0; f < d; ++f) t = fmaf(dZ1[(int64_t)i * dp + f], __ldg(xj + f), t);
+              for (int f = 0; f < d; ++f) t = fmaf(dZ1[(int64_t)j * dp + f], __ldg(xi + f), t);
+              Gd += t;
+            }
+            for (int l = 2; l <= L; ++l) {
+              const float* const dZl = dZ(l); const float* const Hp = Hh(l - 1);
+              float t = 0.f;
+              for (int f = 0; f < hid; ++f) t = fmaf(dZl[(int64_t)i * VW + f], Hp[(int64_t)j * VW + f], t);
+              for (int f = 0; f < hid; ++f) t = fmaf(dZl[(int64_t)j * VW + f], Hp[(int64_t)i * VW + f], t);
+              Gd += t;
+            }
+          } else {   // only the rows of layer l, the two directions added one by one
+            Gd = lapg[p];
+            if (i < R[1]) {
+              float t = 0.f;
+              const float* xr = feat + (int64_t)lo2gid[j] * d;
+              for (int f = 0; f < d; ++f) t = fmaf(dZ1[(int64_t)i * dp + f], __ldg(xr + f), t);
+              Gd += t;
+            }
+            if (j < R[1]) {
+              float t = 0.f;
+              const float* xr = feat + (int64_t)lo2gid[i] * d;
+              for (int f = 0; f < d; ++f) t = fmaf(dZ1[(int64_t)j * dp + f], __ldg(xr + f), t);
+              Gd += t;
+            }
+            for (int l = 2; l <= L; ++l) {
+              const float* const dZl = dZ(l); const float* const Hp = Hh(l - 1);
+              if (i < R[l]) { float t = 0.f; for (int f = 0; f < hid; ++f) t = fmaf(dZl[(int64_t)i * VW + f], Hp[(int64_t)j * VW + f], t); Gd += t; }
+              if (j < R[l]) { float t = 0.f; for (int f = 0; f < hid; ++f) t = fmaf(dZl[(int64_t)j * VW + f], Hp[(int64_t)i * VW + f], t); Gd += t; }
+            }
           }
           Gd *= 0.5f;  // sym_mask = (S + S^T)/2 (explain.py:671)
           float2 Mv = MM[p];
@@ -209,8 +272,8 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
           const float2 Sn = make_float2(sigmoid_fast(Mv.x, ieee), sigmoid_fast(Mv.y, ieee));
           MM[p] = Mv; mm[p] = m2; vv[p] = v2; SS[p] = Sn;
           const float an = 0.5f * (Sn.x + Sn.y);
-          if (i < n2) a[ppij[p]] = an;
-          if (j < n2) a[ppji[p]] = an;
+          if (kGraph || i < n2) a[ppij[p]] = an;
+          if (kGraph || j < n2) a[ppji[p]] = an;
           if (last) { A.out_mask[edge_off + poij[p]] = an; A.out_mask[edge_off + poji[p]] = an; }
         }
       }
@@ -219,33 +282,37 @@ __global__ void __launch_bounds__(kVarThreads) explain_var_kernel(const ExplainA
   }
 }
 
+// calls f(kernel) with the instantiation for the mode and the model
+template <typename F>
+cudaError_t with_var_kernel(int graph_mode, const GxModelDev& m, F&& f) {
+  return var_dispatch(m, [&](auto bn, auto kw) {
+    return graph_mode ? f(explain_var_kernel<true, decltype(bn)::value, decltype(kw)::value>)
+                      : f(explain_var_kernel<false, decltype(bn)::value, decltype(kw)::value>);
+  });
+}
+
 }  // namespace
 
-int gx_var_smem_bytes(int d, int L, int hid, int emb, int C) { return var_smem(d, L, hid, emb, C, kVarThreads / 32).total * 4; }
+// var_smem's carve-up + in graph mode the edge-less rows' constant embedding and the arg-max row of every pooled feature (cst, arg)
+int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C) {
+  const int pool = graph_mode ? 2 * gx_round_up(hid * (L - 1) + emb, 4) : 0;
+  return (var_smem(d, L, hid, emb, C, kVarThreads / 32).total + pool) * 4;
+}
 int gx_var_row_stride(int hid, int emb) { return 32 * var_kw(hid, emb); }
 
-cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, const GxGraphDev& g, const GxModelDev& m,
-                                  const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
+int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m) {
+  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C);
+  int n = 0;
+  with_var_kernel(graph_mode, m, [&](auto kern) { n = var_ctas_per_sm(kern, bytes); return cudaSuccess; });
+  return n;
+}
+
+cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
+                                  const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                   float* out_mask, float* out_feat, cudaStream_t s) {
-  const ExplainArgs args = explain_args(cfg, g, m, hp, plan, m0, out_mask, out_feat);
-  const int bytes = gx_var_smem_bytes(m.d, m.L, m.hid, m.emb, m.C);
-  const int kw = var_kw(m.hid, m.emb);
-  auto go = [&](auto kern) -> cudaError_t {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e != cudaSuccess) return e;
-    // every launch class asks for the largest shared-memory carveout: CTAs of different classes (= different kernels / footprints) can then
-    // share an SM; with per-kernel carveouts a CTA waits for an SM that is completely idle
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e != cudaSuccess) return e;
-    kern<<<cfg.grid, kVarThreads, bytes, s>>>(args);
-    return cudaGetLastError();
-  };
-  if (m.bn) {
-    if (kw == 1) return go(explain_var_kernel<true, 1>);
-    if (kw == 2) return go(explain_var_kernel<true, 2>);
-    return go(explain_var_kernel<true, 4>);
-  }
-  if (kw == 1) return go(explain_var_kernel<false, 1>);
-  if (kw == 2) return go(explain_var_kernel<false, 2>);
-  return go(explain_var_kernel<false, 4>);
+  VarArgs args;
+  fill_queue_args(args, cfg, m, hp, plan, m0, out_mask, out_feat);
+  args.g = g; args.gb = gb; args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
+  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C);
+  return with_var_kernel(graph_mode, m, [&](auto kern) { return var_launch(kern, args, cfg.grid, bytes, s); });
 }

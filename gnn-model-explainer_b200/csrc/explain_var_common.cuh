@@ -1,8 +1,10 @@
-// explain_var_common.cuh -- the per-row and per-parameter steps shared by the two model-variant kernels: explain_var.cu (node tasks)
-// and explain_graph_var.cu (graph classification).  Both are written for clarity, not speed: one warp per row with lane = feature,
-// KW chunks of 32 lanes for widths up to 128 (chunk k holds features 32k + lane), the TRUE widths (no zero padding: a padded column
-// would enter the bn statistics), state in a per-CTA global slab.
+// explain_var_common.cuh -- the per-row and per-parameter steps and the launch code shared by the model-variant kernel
+// (explain_var.cu, node and graph mode) and the unconstrained kernel (explain_dense.cu).  Both are written for clarity, not speed:
+// one persistent CTA per task, one warp per row with lane = feature, KW chunks of 32 lanes for widths up to 128 (chunk k holds
+// features 32k + lane), the TRUE widths (no zero padding: a padded column would enter the bn statistics), state in a per-CTA global slab.
 #pragma once
+#include <type_traits>
+
 #include "explain_common.cuh"
 
 namespace {
@@ -63,6 +65,19 @@ __device__ __forceinline__ void var_stage_model(const GxModelDev& m, const VarSm
 __device__ __forceinline__ float var_init_param(const GxHparamsDev& hp, const float* m0, int64_t m0_idx, uint32_t key, uint32_t slot, float m0_std) {
   if (hp.init == GX_INIT_PHILOX) return 1.0f + m0_std * philox_normal(hp.seed, key, slot);
   return __ldg(m0 + m0_idx);
+}
+
+// Takes the persistent CTA's next task from the work queue (A.order, A.ntasks, A.counter) into task_id; false when the queue is drained.
+// Every thread calls.
+template <typename Args>
+__device__ __forceinline__ bool var_next_task(const Args& A, int& s_task, int tid, int& task_id) {
+  __syncthreads();
+  if (tid == 0) s_task = atomicAdd(A.counter, 1);
+  __syncthreads();
+  const int qi = s_task;
+  if (qi >= A.ntasks) return false;
+  task_id = A.order[qi];
+  return true;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------- forward
@@ -134,6 +149,26 @@ __device__ __forceinline__ float var_activate(const float (&y)[KW], int wout, bo
   }
   return q;
 }
+// Layer l's per-row arrays, as the kernels' slab accessors give them: Yh(l) normalised pre-activations (row stride 32 * KW), H(l) outputs
+// (row stride ldh), qn(l) norms, istd(l) the bn standardisation's 1/std.  The addresses are formed where they are used.
+// Row i of layer l (1 .. L) after its aggregate is in zs: y = b + zs W, var_activate, then the stores (H is 0 in the padding lanes).
+template <bool kBn, int KW, typename YhF, typename HF, typename QF, typename IF>
+__device__ __forceinline__ void var_row_forward(const float* zs, int win, const float* Ws, int wout, const float* bsm, int l, int L, int i,
+                                                YhF Yh, HF H, int64_t ldh, QF qn, IF istd, int lane) {
+  __syncwarp();
+  float y[KW];
+  var_dense<KW>(zs, win, Ws, wout, bsm, y, lane);
+  __syncwarp();
+  float yh[KW], h[KW], is = 1.f;
+  const float q = var_activate<kBn, KW>(y, wout, l < L, yh, h, &is, lane);
+  if (kBn && l < L && lane == 0) istd(l)[i] = is;
+#pragma unroll
+  for (int k = 0; k < KW; ++k) {
+    Yh(l)[(int64_t)i * (32 * KW) + lane + 32 * k] = yh[k];
+    H(l)[(int64_t)i * ldh + lane + 32 * k] = lane + 32 * k < wout ? h[k] : 0.f;
+  }
+  if (lane == 0) qn(l)[i] = q;
+}
 
 // --------------------------------------------------------------------------------------------------------------------------- backward
 // g += (A_m^T dZ_{l+1})[row] over the row's leading columns < bound (A_m symmetric); dZn rows have stride 32 * KW
@@ -179,6 +214,18 @@ __device__ __forceinline__ void var_norm_backward(const float (&g)[KW], const fl
 #pragma unroll
   for (int k = 0; k < KW; ++k)
     if (lane + 32 * k < wout) zs[lane + 32 * k] = (g[k] - yh[k] * sdot) / q;
+}
+// Row i of layer l, g = dL/dH -> zs = dL/dY: the bn and ReLU backward on hidden layers, then the backward of y / max(|y|, eps).
+// H, qn, istd as in var_row_forward.
+template <bool kBn, int KW, typename HF, typename QF, typename IF>
+__device__ __forceinline__ void var_row_backward(float (&g)[KW], const float (&yh)[KW], int l, int L, int i, HF H, int64_t ldh, QF qn, IF istd,
+                                                 int wout, float* zs, int lane) {
+  if (l < L) var_hidden_backward<kBn, KW>(g, yh, H(l) + (int64_t)i * ldh, kBn ? istd(l)[i] : 1.f, wout, lane);
+  const float sdot = var_norm_dot<KW>(g, yh, wout, lane);
+  const float q = qn(l)[i];
+  __syncwarp();
+  var_norm_backward<KW>(g, yh, sdot, q, wout, zs, lane);
+  __syncwarp();
 }
 // layer 1: dZ[f] = sum_c dY[c] W[f][c] for f < d; gFp[f] += dZ[f] U[f] (dL/dsF partial), dZ1row = dZ (.) sF (kept masked for the edge dots)
 __device__ __forceinline__ void var_first_layer_dz(const float* zs, const float* Ws, int d, int wout, const float* Urow, const float* sF,
@@ -255,6 +302,66 @@ __device__ __forceinline__ void var_readout_tail(const float* emb, const float* 
     for (int c = 0; c < C; ++c) t = fmaf(logit[c], Wpp[c * PD + k], t);
     dEmb[k] = t;
   }
+}
+
+// Graph mode's readout input (models.py:283,291,300): pooled feature k = column c of layer l is the max over rows 0 .. n-1 of
+// Hl(l)[i * ld + c], starting from best0[k] (nullptr: -inf) and arg0; arg[k] = the first maximal row, like torch.max.  Every thread calls.
+template <typename Hl>
+__device__ __forceinline__ void var_max_pool(int L, int hid, int PD, int n, Hl Hl_of, int64_t ld, const float* best0, int arg0,
+                                             float* emb, int* arg, int tid, int nt) {
+  for (int k = tid; k < PD; k += nt) {
+    const int l = k < hid * (L - 1) ? k / hid + 1 : L;
+    const int c = k - hid * (l - 1);
+    const float* const H = Hl_of(l);
+    float best = best0 != nullptr ? best0[k] : -INFINITY;
+    int bi = arg0;
+    for (int i = 0; i < n; ++i) {
+      const float v = H[(int64_t)i * ld + c];
+      if (v > best) { best = v; bi = i; }   // strict: the first maximal row wins
+    }
+    emb[k] = best; arg[k] = bi;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------------- launch
+// Calls f(std::integral_constant<bool, kBn>, std::integral_constant<int, KW>) with the model's instantiation.
+template <typename F>
+cudaError_t var_dispatch(const GxModelDev& m, F&& f) {
+  using B = std::integral_constant<bool, true>;
+  using N = std::integral_constant<bool, false>;
+  const int kw = var_kw(m.hid, m.emb);
+  if (m.bn) {
+    if (kw == 1) return f(B(), std::integral_constant<int, 1>());
+    if (kw == 2) return f(B(), std::integral_constant<int, 2>());
+    return f(B(), std::integral_constant<int, 4>());
+  }
+  if (kw == 1) return f(N(), std::integral_constant<int, 1>());
+  if (kw == 2) return f(N(), std::integral_constant<int, 2>());
+  return f(N(), std::integral_constant<int, 4>());
+}
+
+// Lets kern use `bytes` of dynamic shared memory with the largest carveout: CTAs of different launch classes (= different kernels /
+// footprints) can then share an SM; with per-kernel carveouts a CTA waits for an SM that is completely idle
+template <typename Args>
+cudaError_t var_set_smem(void (*kern)(Args), int bytes) {
+  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+}
+template <typename Args>
+cudaError_t var_launch(void (*kern)(Args), const Args& args, int grid, int bytes, cudaStream_t s) {
+  const cudaError_t e = var_set_smem(kern, bytes);
+  if (e != cudaSuccess) return e;
+  kern<<<grid, kVarThreads, bytes, s>>>(args);
+  return cudaGetLastError();
+}
+// co-resident CTAs of kern per SM (sizes the persistent grid); 0 on error
+template <typename Args>
+int var_ctas_per_sm(void (*kern)(Args), int bytes) {
+  int n = 0;
+  cudaError_t e = var_set_smem(kern, bytes);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, kVarThreads, bytes);
+  return e == cudaSuccess ? n : 0;
 }
 
 }  // namespace

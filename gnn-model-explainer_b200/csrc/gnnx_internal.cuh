@@ -200,7 +200,8 @@ __host__ __device__ inline GxStreamLayout gx_make_stream_layout(int n, int n1, i
   return L;
 }
 
-// Global-memory slab of one task in the model-variant kernel (explain_var.cu); every hidden-width array has row stride 32.
+// Global-memory slab of one task in the model-variant kernel (explain_var.cu); hidden-width arrays have row stride vw = 32 * ceil(width / 32).
+// Graph mode computes every one of its n rows with an edge at every layer (n2 = n, e1 = e_d) and has no Laplacian term (np_in = 0).
 struct GxVarLayout {
   int64_t a, U, dZ1, lapg, Yh, H, dZ, q, istd;
   int64_t total_words;
@@ -259,29 +260,6 @@ __host__ __device__ inline GxLayoutG gx_make_layout_graph(int na, int e_d, int n
   L.pi = takei(np); L.pj = takei(np); L.ppij = takei(np); L.ppji = takei(np);
   L.total_words = o;
   return L;
-}
-
-// Global-memory slab of one graph in the graph-mode model-variant kernel (explain_graph_var.cu): every one of the `na` rows with an
-// edge is computed at every layer; hidden-width arrays have row stride vw = 32 * ceil(width / 32).
-struct GxGraphVarLayout {
-  int64_t a, U, dZ1, Yh, H, dZ, q, istd;
-  int64_t total_words;
-};
-__host__ __device__ inline GxGraphVarLayout gx_make_graph_var_layout(int na, int e_d, int d, int L, int vw) {
-  GxGraphVarLayout Lo;
-  const int dp = gx_round_up(d, 4);
-  int64_t o = 0;
-  auto take = [&](int64_t words) { int64_t r = o; o += (words + 3) / 4 * 4; return r; };
-  Lo.a = take(e_d);                           // masked adjacency of every directed edge slot (row-major in the relabelled rows)
-  Lo.U = take((int64_t)na * dp);              // A_m X
-  Lo.dZ1 = take((int64_t)na * dp);            // dL/d(A_m X') (.) sigmoid(feat_mask)
-  Lo.Yh = take((int64_t)L * na * vw);         // per layer: normalised pre-activations
-  Lo.H = take((int64_t)L * na * vw);          // per layer: relu (+ standardisation) output = input of the next layer / the max-pool
-  Lo.dZ = take((int64_t)(L - 1) * na * vw);   // layers 2..L: dL/d(A_m H_{l-1})
-  Lo.q = take((int64_t)L * na);
-  Lo.istd = take((int64_t)L * na);
-  Lo.total_words = o;
-  return Lo;
 }
 
 // Global-memory slab of one task in the unconstrained kernel (explain_dense.cu): the dense n x n state and the per-layer activations of
@@ -377,11 +355,6 @@ cudaError_t gx_launch_explain_gang(const GxExplainLaunch& cfg, const GxGraphDev&
                                    const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                    float* out_mask, float* out_feat, cudaStream_t s);
 int gx_gang_smem_bytes(int d, int hid, int C);
-cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, const GxGraphDev& g, const GxModelDev& m,
-                                  const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
-                                  float* out_mask, float* out_feat, cudaStream_t s);
-int gx_var_smem_bytes(int d, int L, int hid, int emb, int C);
-int gx_var_row_stride(int hid, int emb);
 cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, float* pred, float* emb_out, cudaStream_t s);
 constexpr int GX_STREAM_THREADS = 768;  // 24 warps: 80 registers per thread, 5 KB of cp.async staging per warp
 int gx_explain_max_smem();
@@ -396,11 +369,13 @@ cudaError_t gx_launch_graph_plan(const GxGraphBatchDev& gb, int count, GxPlanArr
 cudaError_t gx_launch_explain_graphs(const GxExplainLaunch& cfg, const GxGraphBatchDev& gb, const GxModelDev& m,
                                      const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0, float* out_mask,
                                      float* out_feat, cudaStream_t s);
-cudaError_t gx_launch_explain_graph_var(const GxExplainLaunch& cfg, const GxGraphBatchDev& gb, const GxModelDev& m,
-                                        const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0, float* out_mask,
-                                        float* out_feat, cudaStream_t s);
-int gx_graph_var_smem_bytes(int d, int L, int hid, int emb, int C);
-int gx_graph_var_ctas_per_sm(const GxModelDev& m);
+// explain_var.cu: the model and optimiser variants, node mode (graph_mode 0, g) or graph mode (gb)
+cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
+                                  const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
+                                  float* out_mask, float* out_feat, cudaStream_t s);
+int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C);
+int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m);
+int gx_var_row_stride(int hid, int emb);
 // explain_dense.cu: Explainer.explain(..., unconstrained=True), node mode (graph_mode 0, g) or graph mode (gb); m0 / out_dense are dense
 // (dense_off[t] = the offset of task t's n_t^2 block), out_mask holds the sub-adjacency slots, x.trace / x.trace_pred optional.
 struct GxDenseIo {

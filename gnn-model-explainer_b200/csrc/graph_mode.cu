@@ -3,7 +3,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <numeric>
 #include <vector>
 
 #include "host.cuh"
@@ -86,7 +85,7 @@ int gx_plan_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int64_
       const GxLayoutG L = gx_make_layout_graph(na, T.e_d, T.npairs, h->m.d, h->m.hid, h->m.emb, h->m.C, kGraphThreads / 32);
       T.smem_bytes = L.total_words * 4;
       if (T.smem_bytes > kGraphCap[kNumGraphClasses - 1]) { gx_set_error("gx_plan_graphs: graph %d needs %d bytes of shared memory", g, T.smem_bytes); return GX_ERR_UNSUPPORTED; }
-    }   // model variants: explain_graph_var.cu keeps a graph in a global slab (smem_bytes 0: one launch class), bounded by max_nodes <= 4096
+    }   // model variants: explain_var.cu keeps a graph in a global slab (smem_bytes 0: one launch class), bounded by max_nodes <= 4096
     tn += na; te += T.e_d; tp += T.npairs;
   }
   for (auto& v : h->class_order) v.clear();
@@ -135,7 +134,7 @@ static int explain_graphs_impl(gx_handle* h, const gx_hparams* hp, gx_memspace s
   const char* who = "gx_explain_graphs";
   if (!h || !hp) { gx_set_error("gx_explain_graphs: NULL argument"); return GX_ERR_INVALID; }
   if (!h->has_gplan) { gx_set_error("gx_explain_graphs: no plan (call gx_plan_graphs)"); return GX_ERR_INVALID; }
-  const bool var = h->m.variant || hp->opt != GX_OPT_ADAM;   // the whole batch through explain_graph_var.cu
+  const bool var = h->m.variant || hp->opt != GX_OPT_ADAM;   // the whole batch through explain_var.cu
   int rc = check_explain_hparams(who, hp, 0, var, io, true);
   if (rc != GX_OK) return rc;
   GX_CUDA_CHECK(cudaSetDevice(h->device));
@@ -153,23 +152,8 @@ static int explain_graphs_impl(gx_handle* h, const gx_hparams* hp, gx_memspace s
   hd.adam_tab = h->d_adam.as<float2>();
   GX_CUDA_CHECK(cudaMemsetAsync(h->d_counters.p, 0, kNumClasses * 4, h->stream));
   if (var) {
-    // one persistent launch over the whole batch, largest graphs first (d_order); per CTA a global slab for one graph and its pair slab
-    if (gx_graph_var_smem_bytes(h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C) > gx_explain_max_smem()) { gx_set_error("gx_explain_graphs: model does not fit the variant kernel"); return GX_ERR_UNSUPPORTED; }
-    const int per_sm = gx_graph_var_ctas_per_sm(h->m);
-    if (per_sm < 1) { gx_set_error("gx_explain_graphs: the variant kernel cannot be resident (%d bytes of shared memory)", gx_graph_var_smem_bytes(h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C)); return GX_ERR_UNSUPPORTED; }
-    const int vw = gx_var_row_stride(h->m.hid, h->m.emb);
-    std::vector<int32_t> all(count);
-    std::iota(all.begin(), all.end(), 0);
-    GxExplainLaunch cfg{};
-    cfg.order = h->d_order.as<int32_t>(); cfg.ntasks = count; cfg.counter = h->d_counters.as<int32_t>(); cfg.x = D.x;
-    rc = size_slab_launch(h, who, all, [&](const GxTask& T) { return gx_make_graph_var_layout(T.n, T.e_d, h->m.d, h->m.L, vw).total_words; },
-                          h->num_sms * per_sm, &cfg);
+    rc = launch_var_batch(h, who, 1, hd, D);
     if (rc != GX_OK) return rc;
-    rc = place_pair_slabs(h, &cfg, &cfg.grid, 1);
-    if (rc == GX_OK) rc = begin_timing(h);
-    if (rc != GX_OK) return rc;
-    GX_CUDA_CHECK(gx_launch_explain_graph_var(cfg, h->gb, h->m, hd, h->plan, D.m0, D.out, D.feat, h->stream));
-    h->launches += 1;
   } else {
     // one persistent launch per footprint class, each requesting its largest footprint, as many CTAs per SM as fit
     GxExplainLaunch cfg[kNumGraphClasses] = {};

@@ -208,6 +208,15 @@ int size_slab_launch(gx_handle* h, const char* who, const std::vector<int32_t>& 
   return GX_OK;
 }
 
+// Words of task T's slab in explain_var.cu (graph mode has no Laplacian term, so no per-pair lapg)
+inline int64_t var_slab_words(const gx_handle* h, int graph_mode, const GxTask& T) {
+  return gx_make_var_layout(T.n, T.n2, T.e1, graph_mode ? 0 : T.npairs_in, h->m.d, h->m.L, gx_var_row_stride(h->m.hid, h->m.emb)).total_words;
+}
+
+// One persistent launch of explain_var.cu over the whole plan (d_order, work-queue counter 0), each CTA with a task slab and a pair
+// slab: at most 4 CTAs per SM in node mode, as many as are co-resident in graph mode.  Records ev_t0 before the launch.
+int launch_var_batch(gx_handle* h, const char* who, int graph_mode, const GxHparamsDev& hd, const IoDev& D);
+
 // Runs the n launch classes of an explain call.  h->class_order[c] holds class c's tasks and d_order holds them class by class; the
 // caller fills cfg[c] with the class's grid, threads, shared memory, cluster / gang size and task slabs, and slabs[c] with its number
 // of pair slabs.  Class c gets its slice of d_order, work-queue counter c and its own pair slabs, and runs on h->side[c], forked from

@@ -4,7 +4,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <numeric>
 #include <vector>
 
 #include "host.cuh"
@@ -346,8 +345,6 @@ static int explain_nodes_impl(gx_handle* h, const gx_hparams* hp, int mode, gx_m
   if (rc != GX_OK) return rc;
   hd.adam_tab = h->d_adam.as<float2>();   // (the buffer may have been (re)allocated by the upload)
   GX_CUDA_CHECK(cudaMemsetAsync(h->d_counters.p, 0, kNumClasses * 4, h->stream));
-  const int vw = gx_var_row_stride(h->m.hid, h->m.emb);
-  auto var_words = [&](const GxTask& T) { return gx_make_var_layout(T.n, T.n2, T.e1, T.npairs_in, h->m.d, h->m.L, vw).total_words; };
   auto outer_pairs = [&]() -> int {
     // pairs between two outermost nodes: independent scalar recurrences, whole batch in one launch
     GX_CUDA_CHECK(gx_launch_outer_pairs(hd, h->g, h->plan, count, D.m0, D.out, D.x, h->stream));
@@ -356,97 +353,84 @@ static int explain_nodes_impl(gx_handle* h, const gx_hparams* hp, int mode, gx_m
   };
   if (all_var && !h->m.variant) {
     // default model, optimiser other than Adam: the whole batch in one launch of the variant kernel (+ the outer-pair recurrences)
-    if (gx_var_smem_bytes(h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C) > gx_explain_max_smem()) { gx_set_error("gx_explain_nodes: model does not fit the variant kernel"); return GX_ERR_UNSUPPORTED; }
-    std::vector<int32_t> all(count);
-    std::iota(all.begin(), all.end(), 0);
-    GxExplainLaunch cfg{};
-    cfg.order = h->d_order.as<int32_t>(); cfg.ntasks = count; cfg.counter = h->d_counters.as<int32_t>(); cfg.x = D.x;
-    rc = size_slab_launch(h, who, all, var_words, h->num_sms * 4, &cfg);
+    rc = launch_var_batch(h, who, 0, hd, D);
+    if (rc == GX_OK) rc = outer_pairs();
     if (rc != GX_OK) return rc;
-    rc = place_pair_slabs(h, &cfg, &cfg.grid, 1);
-    if (rc == GX_OK) rc = begin_timing(h);
-    if (rc != GX_OK) return rc;
-    GX_CUDA_CHECK(gx_launch_explain_var(cfg, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, h->stream));
-    h->launches += 1;
-    rc = outer_pairs();
-    if (rc != GX_OK) return rc;
-    GX_CUDA_CHECK(cudaEventRecord(h->ev_t1, h->stream));
-    h->timed = true;
-    return io_finish(h, hp, space, io, count, te, h->m.d, h->m.C, D);
-  }
-  // per launch class: its kernel, grid, block and shared memory (the largest footprint of its tasks) and its number of pair slabs
-  GxExplainLaunch cfg[kNumClasses] = {};
-  int slabs[kNumClasses] = {};
-  NodeKernel kernel[kNumClasses] = {};
-  for (int c = 0; c < kNumClasses; ++c) {
-    const LaunchClass& K = h->classes[c];
-    const int nt = (int)h->class_order[c].size();
-    int need = 0;
-    for (int32_t t : h->class_order[c]) need = std::max(need, h->tasks[t].smem_bytes);
-    cfg[c].threads = K.threads;
-    cfg[c].dbg = h->dbg;
-    cfg[c].x = D.x;
-    if (c == kClusterClass) {
-      // CTAs, CS per task, one pair slab per cluster; the class requests the whole SM (see the 1-per-SM class)
-      kernel[c] = NodeKernel::cluster;
-      cfg[c].cluster = h->plan_cluster;
-      cfg[c].grid = std::min<int>(nt, h->num_sms / h->plan_cluster) * h->plan_cluster;
-      cfg[c].smem_bytes = std::max(need, K.cap_bytes - 2048);
-      slabs[c] = cfg[c].grid / h->plan_cluster;
-    } else if (K.cap_bytes > 0) {
-      // the dynamic shared memory request shrinks to what the class needs (more CTAs can co-reside).  The 1-per-SM class requests
-      // the whole SM: a CTA of another class next to it would take the room the scheduler's breadth-first placement needs for the
-      // small classes launched last (2 KB short of the class limit: kernels with a trace carry 1.2 KB of static shared memory)
-      kernel[c] = NodeKernel::smem;
-      cfg[c].grid = std::min<int>(nt, h->num_sms * K.ctas_per_sm);
-      cfg[c].smem_bytes = c == kOneClass ? std::max(need, K.cap_bytes - 2048) : std::max(need, 1024);
-      slabs[c] = cfg[c].grid;
-    } else if (nt > 0) {
-      // slab class: as many tasks in flight as the device memory holds, up to one per SM (CTAs of explain_stream.cu / explain_var.cu,
-      // gangs of explain_gang.cu)
-      int max_slabs = h->num_sms, gang = 0;   // gang > 0: explain_gang.cu with this many CTAs per task
-      if (!h->m.variant && h->gang_override >= 0 && h->m.d <= 128 && gx_gang_smem_bytes(h->m.d, h->m.hid, h->m.C) <= gx_explain_max_smem()) {
-        // explain_gang.cu: G co-resident CTAs per task.  As many tasks in flight as keep their randomly accessed state
-        // (a, gE: 8 B per directed edge; P, dP, dY1: 240 B per node) inside 5/8 of the L2 (31 MB of an H100's 50 MB), the SMs
-        // divided evenly among them.
-        int64_t ws = 1;
-        for (int32_t t : h->class_order[c]) ws = std::max<int64_t>(ws, (int64_t)h->tasks[t].e_d * 8 + (int64_t)h->tasks[t].n * 240);
-        const int64_t l2_budget = h->l2_bytes * 5 / 8;
-        int ngangs = (int)std::max<int64_t>(1, std::min<int64_t>(std::min(nt, h->num_sms), l2_budget / ws));
-        gang = std::max(1, std::min(h->num_sms / ngangs, GX_MAX_GANG));
-        if (h->gang_override > 0) gang = std::min(std::min(h->gang_override, h->num_sms), GX_MAX_GANG);
-        max_slabs = std::max(1, std::min(ngangs, h->num_sms / gang));
-      }
-      kernel[c] = h->m.variant ? NodeKernel::variant : gang > 0 ? NodeKernel::gang : NodeKernel::stream1;
-      auto stream_words = [&](const GxTask& T) { return gx_make_stream_layout(T.n, T.n1, T.n2, T.e_d, T.npairs_in, h->m.d, h->m.hid, GX_STREAM_THREADS / 32).total_words; };
-      rc = h->m.variant ? size_slab_launch(h, who, h->class_order[c], var_words, max_slabs, &cfg[c])
-                        : size_slab_launch(h, who, h->class_order[c], stream_words, max_slabs, &cfg[c]);
-      if (rc != GX_OK) return rc;
-      slabs[c] = cfg[c].grid;
-      if (gang > 0) {
-        cfg[c].gang = gang;
-        cfg[c].grid = slabs[c] * gang;
-        GX_CUDA_CHECK(h->d_gang.reserve((size_t)slabs[c] * 16));
-        cfg[c].gang_bars = h->d_gang.as<unsigned long long>();
-        cfg[c].gang_mail = reinterpret_cast<int32_t*>(h->d_gang.as<char>() + (size_t)slabs[c] * 8);
+  } else {
+    // per launch class: its kernel, grid, block and shared memory (the largest footprint of its tasks) and its number of pair slabs
+    GxExplainLaunch cfg[kNumClasses] = {};
+    int slabs[kNumClasses] = {};
+    NodeKernel kernel[kNumClasses] = {};
+    for (int c = 0; c < kNumClasses; ++c) {
+      const LaunchClass& K = h->classes[c];
+      const int nt = (int)h->class_order[c].size();
+      int need = 0;
+      for (int32_t t : h->class_order[c]) need = std::max(need, h->tasks[t].smem_bytes);
+      cfg[c].threads = K.threads;
+      cfg[c].dbg = h->dbg;
+      cfg[c].x = D.x;
+      if (c == kClusterClass) {
+        // CTAs, CS per task, one pair slab per cluster; the class requests the whole SM (see the 1-per-SM class)
+        kernel[c] = NodeKernel::cluster;
+        cfg[c].cluster = h->plan_cluster;
+        cfg[c].grid = std::min<int>(nt, h->num_sms / h->plan_cluster) * h->plan_cluster;
+        cfg[c].smem_bytes = std::max(need, K.cap_bytes - 2048);
+        slabs[c] = cfg[c].grid / h->plan_cluster;
+      } else if (K.cap_bytes > 0) {
+        // the dynamic shared memory request shrinks to what the class needs (more CTAs can co-reside).  The 1-per-SM class requests
+        // the whole SM: a CTA of another class next to it would take the room the scheduler's breadth-first placement needs for the
+        // small classes launched last (2 KB short of the class limit: kernels with a trace carry 1.2 KB of static shared memory)
+        kernel[c] = NodeKernel::smem;
+        cfg[c].grid = std::min<int>(nt, h->num_sms * K.ctas_per_sm);
+        cfg[c].smem_bytes = c == kOneClass ? std::max(need, K.cap_bytes - 2048) : std::max(need, 1024);
+        slabs[c] = cfg[c].grid;
+      } else if (nt > 0) {
+        // slab class: as many tasks in flight as the device memory holds, up to one per SM (CTAs of explain_stream.cu / explain_var.cu,
+        // gangs of explain_gang.cu)
+        int max_slabs = h->num_sms, gang = 0;   // gang > 0: explain_gang.cu with this many CTAs per task
+        if (!h->m.variant && h->gang_override >= 0 && h->m.d <= 128 && gx_gang_smem_bytes(h->m.d, h->m.hid, h->m.C) <= gx_explain_max_smem()) {
+          // explain_gang.cu: G co-resident CTAs per task.  As many tasks in flight as keep their randomly accessed state
+          // (a, gE: 8 B per directed edge; P, dP, dY1: 240 B per node) inside 5/8 of the L2 (31 MB of an H100's 50 MB), the SMs
+          // divided evenly among them.
+          int64_t ws = 1;
+          for (int32_t t : h->class_order[c]) ws = std::max<int64_t>(ws, (int64_t)h->tasks[t].e_d * 8 + (int64_t)h->tasks[t].n * 240);
+          const int64_t l2_budget = h->l2_bytes * 5 / 8;
+          int ngangs = (int)std::max<int64_t>(1, std::min<int64_t>(std::min(nt, h->num_sms), l2_budget / ws));
+          gang = std::max(1, std::min(h->num_sms / ngangs, GX_MAX_GANG));
+          if (h->gang_override > 0) gang = std::min(std::min(h->gang_override, h->num_sms), GX_MAX_GANG);
+          max_slabs = std::max(1, std::min(ngangs, h->num_sms / gang));
+        }
+        kernel[c] = h->m.variant ? NodeKernel::variant : gang > 0 ? NodeKernel::gang : NodeKernel::stream1;
+        auto stream_words = [&](const GxTask& T) { return gx_make_stream_layout(T.n, T.n1, T.n2, T.e_d, T.npairs_in, h->m.d, h->m.hid, GX_STREAM_THREADS / 32).total_words; };
+        rc = h->m.variant ? size_slab_launch(h, who, h->class_order[c], [&](const GxTask& T) { return var_slab_words(h, 0, T); }, max_slabs, &cfg[c])
+                          : size_slab_launch(h, who, h->class_order[c], stream_words, max_slabs, &cfg[c]);
+        if (rc != GX_OK) return rc;
+        slabs[c] = cfg[c].grid;
+        if (gang > 0) {
+          cfg[c].gang = gang;
+          cfg[c].grid = slabs[c] * gang;
+          GX_CUDA_CHECK(h->d_gang.reserve((size_t)slabs[c] * 16));
+          cfg[c].gang_bars = h->d_gang.as<unsigned long long>();
+          cfg[c].gang_mail = reinterpret_cast<int32_t*>(h->d_gang.as<char>() + (size_t)slabs[c] * 8);
+        }
       }
     }
-  }
-  auto launch = [&](int c, const GxExplainLaunch& k, cudaStream_t s) -> cudaError_t {
-    switch (kernel[c]) {
-      case NodeKernel::smem:
-      case NodeKernel::cluster: return gx_launch_explain(k, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
-      case NodeKernel::variant: return gx_launch_explain_var(k, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
-      case NodeKernel::stream1: return gx_launch_explain_stream(k, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
-      case NodeKernel::gang: {
-        const cudaError_t e = cudaMemsetAsync(k.gang_bars, 0, (size_t)(k.grid / k.gang) * 16, s);
-        return e != cudaSuccess ? e : gx_launch_explain_gang(k, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
+    auto launch = [&](int c, const GxExplainLaunch& k, cudaStream_t s) -> cudaError_t {
+      switch (kernel[c]) {
+        case NodeKernel::smem:
+        case NodeKernel::cluster: return gx_launch_explain(k, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
+        case NodeKernel::variant: return gx_launch_explain_var(k, 0, h->g, h->gb, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
+        case NodeKernel::stream1: return gx_launch_explain_stream(k, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
+        case NodeKernel::gang: {
+          const cudaError_t e = cudaMemsetAsync(k.gang_bars, 0, (size_t)(k.grid / k.gang) * 16, s);
+          return e != cudaSuccess ? e : gx_launch_explain_gang(k, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
+        }
       }
-    }
-    return cudaErrorInvalidValue;
-  };
-  rc = launch_classes(h, kNumClasses, cfg, slabs, launch, outer_pairs);
-  if (rc != GX_OK) return rc;
+      return cudaErrorInvalidValue;
+    };
+    rc = launch_classes(h, kNumClasses, cfg, slabs, launch, outer_pairs);
+    if (rc != GX_OK) return rc;
+  }
   if (D.x.trace) {
     GX_CUDA_CHECK(gx_launch_trace_finalize(hd, h->plan, count, D.x, h->stream));
     h->launches += 1;

@@ -1,4 +1,4 @@
-"""GPU (-m gpu): graph-classification mode (explain_graph.cu, explain_graph_var.cu) where the 12 golden graphs never take it: feature
+"""GPU (-m gpu): graph-classification mode (explain_graph.cu, explain_var.cu) where the 12 golden graphs never take it: feature
 masks, inputs wider than 32 features (lane groups of 9..32 lanes), more than 32 classes with pred_model read from global memory, every
 shared-memory launch class up to the largest graph the tuned kernel accepts, structural edge cases of the max-pool, the benchmarked batch,
 one teacher-forced step, and the device Philox init against its host restatement in every kernel.

@@ -1,4 +1,4 @@
-"""GPU (-m gpu): graph-classification mode with the model and optimiser variants (explain_graph_var.cu through the C ABI and the
+"""GPU (-m gpu): graph-classification mode with the model and optimiser variants (explain_var.cu in graph mode, through the C ABI and the
 drop-in Explainer), against the masks the UNMODIFIED reference returned (tests/golden/graph_variants_golden.npz, 30 epochs) and
 against the line-by-line torch port on random models, a graph larger than the tuned kernel's shared memory, and the tuned kernel."""
 import os

@@ -1,4 +1,4 @@
-"""bench_graph_variants.py -- graphs/s of graph-classification mode with model variants (csrc/explain_graph_var.cu).
+"""bench_graph_variants.py -- graphs/s of graph-classification mode with model variants (csrc/explain_var.cu, graph mode).
 
     python tools/bench_graph_variants.py [--steps K] [--warmup W]
 
@@ -33,7 +33,7 @@ def _gpu_name_power(index):
 
 
 def bench_graph_variants(a, c, adj, feat, label):
-    """The same stand-in explained with model variants (explain_graph_var.cu): a 3-layer --bn model and a 4-layer model (hidden /
+    """The same stand-in explained with model variants (explain_var.cu): a 3-layer --bn model and a 4-layer model (hidden /
     output 20, random weights), Philox init, 100 epochs.  Device time of the explain call (CUDA events), graphs/s."""
     import ctypes as C
     import gnnx
@@ -68,7 +68,7 @@ def bench_graph_variants(a, c, adj, feat, label):
         ms, _, _, _ = timed(c, step, steps, warmup)
         eng.close()
         out[tag] = {"value": G * steps / (ms / 1e3), "unit": "graphs/s", "ms_per_step": ms / steps, "steps": steps, "warmup": warmup,
-                    "num_layers": L, "bn": bn, "hidden_dim": 20, "output_dim": 20, "kernel": "explain_graph_var_kernel",
+                    "num_layers": L, "bn": bn, "hidden_dim": 20, "output_dim": 20, "kernel": "explain_var_kernel",
                     "gpu": name, "power_limit_w": power, "timing": "CUDA events around gx_explain_graphs (plan outside), L2 flushed between steps"}
     return out
 

@@ -76,6 +76,15 @@ def main():
         eng.explain_nodes_host(eng.make_hparams(num_epochs=EPOCHS, opt=1), util.golden_m0(fx, plan), out)
         print("var ok sgd", float(out.sum()))
         eng.close()
+        gg = np.load(util.GOLDEN + "/graphs_golden.npz")   # graph mode: the default model with SGD -> the variant kernel
+        eng = gnnx.Engine(0)
+        eng.set_model({k: gg[k] for k in util.WKEYS})
+        eng.set_graph_batch(gg["adj"], gg["feat"], gg["label"])
+        eoff = eng.plan_graphs([0, 3, 5])
+        out = np.zeros(int(eoff[-1]), np.float32)
+        eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS, opt=1, init=_abi.GX_INIT_PHILOX, seed=3), None, out)
+        print("var ok graph sgd", float(out.sum()))
+        eng.close()
     if "cluster" in which:
         eng = util.make_engine(fx)
         eng.debug_cluster(4, 1)
