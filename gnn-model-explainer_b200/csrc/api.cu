@@ -203,7 +203,7 @@ int place_pair_slabs(gx_handle* h, GxExplainLaunch* cfg, const int* slabs, int n
 }
 
 int launch_var_batch(gx_handle* h, const char* who, int graph_mode, const GxHparamsDev& hd, const IoDev& D) {
-  const int bytes = gx_var_smem_bytes(graph_mode, h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C);
+  const int bytes = gx_var_smem_bytes(graph_mode, h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C, h->m.att);
   if (bytes > gx_explain_max_smem()) { gx_set_error("%s: model does not fit the variant kernel", who); return GX_ERR_UNSUPPORTED; }
   int max_ctas = h->num_sms * 4;
   if (graph_mode) {   // graph mode: as many CTAs as are co-resident
@@ -221,6 +221,66 @@ int launch_var_batch(gx_handle* h, const char* who, int graph_mode, const GxHpar
   if (rc != GX_OK) return rc;
   GX_CUDA_CHECK(gx_launch_explain_var(cfg, graph_mode, h->g, h->gb, h->m, hd, h->plan, D.m0, D.out, D.feat, h->stream));
   h->launches += 1;
+  return GX_OK;
+}
+
+// Model variant (num_gc_layers 2 / 4, --bn, widths 33..128, attention): explain_var.cu, true widths (a zero-padded column would enter
+// the bn statistics).  att_w != nullptr: an attention model, each layer's (in, in) attention weights right after its conv weights
+// (gx_att_weight).  The widths were checked by the caller.
+static int set_variant_model(gx_handle* h, const char* who, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
+                             const float* const* att_w, const float* pred_w, const float* pred_b) {
+  const int L = dims->num_layers, d = dims->input_dim, hid0 = dims->hidden_dim, emb0 = dims->embed_dim, C = dims->num_classes;
+  const int att = att_w != nullptr ? 1 : 0;
+  if (gx_var_smem_bytes(0, d, L, hid0, emb0, C, att) > gx_explain_max_smem()) {
+    gx_set_error("%s: model variant does not fit shared memory", who);
+    return GX_ERR_UNSUPPORTED;
+  }
+  std::vector<float> host;
+  size_t offW[GX_MAX_LAYERS], offb[GX_MAX_LAYERS];
+  auto al4 = [&]() { while (host.size() % 4) host.push_back(0.f); };
+  for (int l = 0; l < L; ++l) {
+    if (!conv_w[l]) { gx_set_error("%s: conv_w[%d] is NULL", who, l); return GX_ERR_INVALID; }
+    if (att && !att_w[l]) { gx_set_error("%s: att_w[%d] is NULL", who, l); return GX_ERR_INVALID; }
+    const int win = l == 0 ? d : hid0, wout = l == L - 1 ? emb0 : hid0;
+    al4(); offW[l] = host.size();
+    host.insert(host.end(), conv_w[l], conv_w[l] + (size_t)win * wout);
+    if (att) host.insert(host.end(), att_w[l], att_w[l] + (size_t)win * win);
+    al4(); offb[l] = host.size();
+    for (int c = 0; c < wout; ++c) host.push_back((conv_b && conv_b[l]) ? conv_b[l][c] : 0.f);
+  }
+  const int PD0 = hid0 * (L - 1) + emb0;
+  al4(); const size_t offWp = host.size();
+  host.insert(host.end(), pred_w, pred_w + (size_t)C * PD0);
+  al4(); const size_t offbp = host.size();
+  host.insert(host.end(), pred_b, pred_b + C);
+  GX_CUDA_CHECK(h->m_buf.reserve(host.size() * 4));
+  GX_CUDA_CHECK(cudaMemcpyAsync(h->m_buf.p, host.data(), host.size() * 4, cudaMemcpyHostToDevice, h->stream));
+  GX_CUDA_CHECK(cudaStreamSynchronize(h->stream));
+  float* b = h->m_buf.as<float>();
+  h->m = GxModelDev{};
+  h->m.d = d; h->m.hid = hid0; h->m.emb = emb0; h->m.C = C; h->m.L = L;
+  h->m.bn = (dims->flags & GX_MODEL_BN) ? 1 : 0; h->m.variant = 1; h->m.att = att;
+  for (int l = 0; l < L; ++l) { h->m.W[l] = b + offW[l]; h->m.Wt[l] = nullptr; h->m.b[l] = b + offb[l]; }
+  h->m.Wp = b + offWp; h->m.bp = b + offbp;
+  h->has_model = true; h->has_plan = false;
+  return GX_OK;
+}
+
+// The dimension checks of gx_set_model / gx_set_model_att
+static int check_model_dims(const char* who, const gx_model_dims* dims) {
+  if (dims->num_layers < 2 || dims->num_layers > GX_MAX_LAYERS) {
+    gx_set_error("%s: num_layers=%d outside [2,%d]", who, dims->num_layers, GX_MAX_LAYERS);
+    return GX_ERR_UNSUPPORTED;
+  }
+  if (dims->hidden_dim < 1 || dims->embed_dim < 1 || dims->hidden_dim > 128 || dims->embed_dim > 128) {
+    gx_set_error("%s: hidden_dim=%d output_dim=%d; this build supports widths up to 128 (tuned kernels up to 32, the variant kernel beyond)", who, dims->hidden_dim, dims->embed_dim);
+    return GX_ERR_UNSUPPORTED;
+  }
+  if (dims->input_dim < 1 || dims->input_dim > 128) {
+    gx_set_error("%s: input_dim=%d outside [1,128] supported by the shared-memory kernel", who, dims->input_dim);
+    return GX_ERR_UNSUPPORTED;
+  }
+  if (dims->num_classes < 1) { gx_set_error("%s: num_classes < 1", who); return GX_ERR_INVALID; }
   return GX_OK;
 }
 
@@ -337,11 +397,13 @@ int gx_model_forward(gx_handle* h, gx_memspace space, float* pred) {
   if (h->m.hid > 32 || h->m.emb > 32) { gx_set_error("gx_model_forward: widths > 32 are not built (pass pred to the Explainer)"); return GX_ERR_UNSUPPORTED; }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
   const size_t np_ = (size_t)h->g.N * h->m.C;
-  GX_CUDA_CHECK(h->d_fwd.reserve(((size_t)h->m.L * h->g.N * 32 + np_) * 4));
+  const size_t npw = h->m.att ? (size_t)h->g.N * gx_round_up(std::max(h->m.d, h->m.hid), 4) : 0;   // attention models: P
+  GX_CUDA_CHECK(h->d_fwd.reserve(((size_t)h->m.L * h->g.N * 32 + np_ + npw) * 4));
   float* H = h->d_fwd.as<float>();
   float* pd = space == GX_DEVICE ? pred : H + (size_t)h->m.L * h->g.N * 32;
-  GX_CUDA_CHECK(gx_launch_model_forward(h->g, h->m, H, pd, nullptr, h->stream));
-  h->launches += h->m.L + 1;
+  float* P = h->m.att ? H + (size_t)h->m.L * h->g.N * 32 + np_ : nullptr;
+  GX_CUDA_CHECK(gx_launch_model_forward(h->g, h->m, H, pd, nullptr, P, h->stream));
+  h->launches += h->m.L * (h->m.att ? 2 : 1) + 1;
   if (space != GX_DEVICE) {
     GX_CUDA_CHECK(cudaMemcpyAsync(pred, pd, np_ * 4, cudaMemcpyDeviceToHost, h->stream));
     GX_CUDA_CHECK(cudaStreamSynchronize(h->stream));
@@ -383,52 +445,12 @@ int gx_last_class_ms(gx_handle* h, float begin_ms[7], float end_ms[7]) {
 int gx_set_model(gx_handle* h, const gx_model_dims* dims, const float* const* conv_w,
                  const float* const* conv_b, const float* pred_w, const float* pred_b) {
   if (!h || !dims || !conv_w || !pred_w || !pred_b) { gx_set_error("gx_set_model: NULL argument"); return GX_ERR_INVALID; }
-  if (dims->num_layers < 2 || dims->num_layers > GX_MAX_LAYERS) {
-    gx_set_error("gx_set_model: num_layers=%d outside [2,%d]", dims->num_layers, GX_MAX_LAYERS);
-    return GX_ERR_UNSUPPORTED;
-  }
-  if (dims->hidden_dim < 1 || dims->embed_dim < 1 || dims->hidden_dim > 128 || dims->embed_dim > 128) {
-    gx_set_error("gx_set_model: hidden_dim=%d output_dim=%d; this build supports widths up to 128 (tuned kernels up to 32, the variant kernel beyond)", dims->hidden_dim, dims->embed_dim);
-    return GX_ERR_UNSUPPORTED;
-  }
-  if (dims->input_dim < 1 || dims->input_dim > 128) {
-    gx_set_error("gx_set_model: input_dim=%d outside [1,128] supported by the shared-memory kernel", dims->input_dim);
-    return GX_ERR_UNSUPPORTED;
-  }
-  if (dims->num_classes < 1) { gx_set_error("gx_set_model: num_classes < 1"); return GX_ERR_INVALID; }
+  const int rc = check_model_dims("gx_set_model", dims);
+  if (rc != GX_OK) return rc;
+  if (dims->flags & GX_MODEL_ATT) { gx_set_error("gx_set_model: GX_MODEL_ATT models are set with gx_set_model_att (it takes the attention weights)"); return GX_ERR_INVALID; }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
-  if (dims->num_layers != 3 || (dims->flags & GX_MODEL_BN) || dims->hidden_dim > 32 || dims->embed_dim > 32) {
-    // Model variant (num_gc_layers 2 / 4, --bn, widths 33..128): explain_var.cu, true widths (a zero-padded column would enter the bn statistics).
-    const int L = dims->num_layers, d = dims->input_dim, hid0 = dims->hidden_dim, emb0 = dims->embed_dim, C = dims->num_classes;
-    if (gx_var_smem_bytes(0, d, L, hid0, emb0, C) > gx_explain_max_smem()) { gx_set_error("gx_set_model: model variant does not fit shared memory"); return GX_ERR_UNSUPPORTED; }
-    std::vector<float> host;
-    size_t offW[GX_MAX_LAYERS], offb[GX_MAX_LAYERS];
-    auto al4 = [&]() { while (host.size() % 4) host.push_back(0.f); };
-    for (int l = 0; l < L; ++l) {
-      if (!conv_w[l]) { gx_set_error("gx_set_model: conv_w[%d] is NULL", l); return GX_ERR_INVALID; }
-      const int win = l == 0 ? d : hid0, wout = l == L - 1 ? emb0 : hid0;
-      al4(); offW[l] = host.size();
-      host.insert(host.end(), conv_w[l], conv_w[l] + (size_t)win * wout);
-      al4(); offb[l] = host.size();
-      for (int c = 0; c < wout; ++c) host.push_back((conv_b && conv_b[l]) ? conv_b[l][c] : 0.f);
-    }
-    const int PD0 = hid0 * (L - 1) + emb0;
-    al4(); const size_t offWp = host.size();
-    host.insert(host.end(), pred_w, pred_w + (size_t)C * PD0);
-    al4(); const size_t offbp = host.size();
-    host.insert(host.end(), pred_b, pred_b + C);
-    GX_CUDA_CHECK(h->m_buf.reserve(host.size() * 4));
-    GX_CUDA_CHECK(cudaMemcpyAsync(h->m_buf.p, host.data(), host.size() * 4, cudaMemcpyHostToDevice, h->stream));
-    GX_CUDA_CHECK(cudaStreamSynchronize(h->stream));
-    float* b = h->m_buf.as<float>();
-    h->m = GxModelDev{};
-    h->m.d = d; h->m.hid = hid0; h->m.emb = emb0; h->m.C = C; h->m.L = L;
-    h->m.bn = (dims->flags & GX_MODEL_BN) ? 1 : 0; h->m.variant = 1;
-    for (int l = 0; l < L; ++l) { h->m.W[l] = b + offW[l]; h->m.Wt[l] = nullptr; h->m.b[l] = b + offb[l]; }
-    h->m.Wp = b + offWp; h->m.bp = b + offbp;
-    h->has_model = true; h->has_plan = false;
-    return GX_OK;
-  }
+  if (dims->num_layers != 3 || (dims->flags & GX_MODEL_BN) || dims->hidden_dim > 32 || dims->embed_dim > 32)
+    return set_variant_model(h, "gx_set_model", dims, conv_w, conv_b, nullptr, pred_w, pred_b);
   // The kernels are instantiated for the reference default 20/20 and for 32/32; any other width <= 32 is
   // zero-padded to 32.  Padding is exact: a padded output column is 0*W + 0 = 0, contributes nothing to the
   // row norm, stays 0 through normalise/ReLU, and its pred_model column is 0 (forward and backward).
@@ -472,6 +494,15 @@ int gx_set_model(gx_handle* h, const gx_model_dims* dims, const float* const* co
   h->has_model = true;
   h->has_plan = false;
   return GX_OK;
+}
+
+int gx_set_model_att(gx_handle* h, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
+                     const float* const* att_w, const float* pred_w, const float* pred_b) {
+  if (!h || !dims || !conv_w || !att_w || !pred_w || !pred_b) { gx_set_error("gx_set_model_att: NULL argument"); return GX_ERR_INVALID; }
+  const int rc = check_model_dims("gx_set_model_att", dims);
+  if (rc != GX_OK) return rc;
+  GX_CUDA_CHECK(cudaSetDevice(h->device));
+  return set_variant_model(h, "gx_set_model_att", dims, conv_w, conv_b, att_w, pred_w, pred_b);
 }
 
 int gx_set_graph_csr(gx_handle* h, int64_t N, const int32_t* rowptr, const int32_t* col,

@@ -19,6 +19,11 @@
 // (GxVarLayout, L2 resident for the reference's graph sizes), one warp per row with lane = feature, one thread per undirected edge in
 // the edge phase.  Phases per epoch (one __syncthreads each): F1 .. FL | (graph mode: pool) | S | BL .. B1 | P.  The default model
 // (3 layers, no bn) with Adam never comes here.
+// Attention models (kAtt, --method att, models.py:62-68) weight every layer's masked adjacency by s_ij = P_i . P_j, P = H_{l-1} Wa_l
+// (unnormalised, no softmax; every layer starts from the masked adjacency).  Per layer the forward adds a projection and an edge
+// phase before the gather (Fl = Pl | Sl | gather with a s); the backward adds, after the row phase, t_ij = dL/dZ_i . H_{l-1}[j] per
+// slot, the pair weights a_ij (t_ij + t_ji), and dL/dP = sum_j a_ij (t_ij + t_ji) P_j, whose dL/dP Wa^T joins dL/dH_{l-1} (layer 1:
+// dL/dsF).  The edge phase then uses dL/da_ij + dL/da_ji = sum_l s_ij (t_ij + t_ji) from the stored s and t.
 #include "explain_var_common.cuh"
 
 namespace {
@@ -41,9 +46,119 @@ struct VarArgs {
   float* out_feat;
 };
 
+// ---------------------------------------------------------------------------------------------------------------- attention layers
+// Forward of one attention layer (every thread calls; ends with __syncthreads).  P = H_{l-1} Wa (row stride ldp) on the layer's
+// nin input rows, H_0 = X (.) sF from the feature rows on layer 1 (Hp == nullptr), else Hp (row stride vw); then s_ij = P_i . P_j and
+// a_ij s_ij on the slots of the rows < min(nin, nsrows) (the rows with stored slots) whose column is an input row.  s_ij and s_ji
+// are the same products summed in the same order, so they are equal.
+__device__ __forceinline__ void att_forward_edges(int win, int ldp, int nin, int nsrows, int d, const float* feat, const int32_t* __restrict__ lo2gid,
+                                                  const float* sF, const float* Hp, int vw, const float* Wa, const int32_t* __restrict__ irp,
+                                                  const int32_t* __restrict__ icol, const float* a, float* P, float* s, float* as, float* zs,
+                                                  int warp, int nwarps, int lane) {
+  for (int i = warp; i < nin; i += nwarps) {
+    if (Hp == nullptr) {
+      const float* const x = feat + (int64_t)lo2gid[i] * d;
+      for (int f = lane; f < d; f += 32) zs[f] = __ldg(x + f) * sF[f];   // x * sigmoid(feat_mask) (explain.py:707)
+    } else {
+      for (int f = lane; f < win; f += 32) zs[f] = Hp[(int64_t)i * vw + f];
+    }
+    __syncwarp();
+    for (int c = lane; c < win; c += 32) {
+      float p = 0.f;
+      for (int f = 0; f < win; ++f) p = fmaf(zs[f], Wa[f * win + c], p);
+      P[(int64_t)i * ldp + c] = p;
+    }
+    __syncwarp();
+  }
+  __syncthreads();
+  const int srows = nin < nsrows ? nin : nsrows;
+  for (int i = warp; i < srows; i += nwarps) {
+    const float* const Pi = P + (int64_t)i * ldp;
+    for (int e = irp[i] + lane; e < irp[i + 1]; e += 32) {
+      const int j = icol[e];
+      if (j >= nin) continue;
+      const float* const Pj = P + (int64_t)j * ldp;
+      float sv = 0.f;
+      for (int f = 0; f < win; ++f) sv = fmaf(Pi[f], Pj[f], sv);
+      s[e] = sv;
+      as[e] = a[e] * sv;
+    }
+  }
+  __syncthreads();
+}
+
+// Backward of one attention layer after its row phase (every thread calls; ends with __syncthreads).  D = dL/dZ of the layer's nrow
+// rows: dZ1 = dL/dZ (.) sF (row stride dp) dotted with the raw feature rows on layer 1 (Hp == nullptr), else dZ_l dotted with
+// Hp = H_{l-1} (row stride vw).
+//   t_ij = D_i . H_{l-1}[j] on every slot of the layer's rows;
+//   cw_ij = cw_ji = a_ij (t_ij + t_ji) per pair (t only where the row is a row of the layer);
+//   dL/dP_i = sum_j cw_ij P_j on the nin input rows (a row beyond the layer's rows has only its leading columns inside them);
+//   dL/dP_i Wa^T -> dHa (the layer below adds it to dL/dH) or, on layer 1, dL/dsF += X (.) dL/dP Wa^T into this warp's partials gFw.
+__device__ __forceinline__ void att_backward_edges(int win, int ldp, int nrow, int nin, int nsrows, int np, int d, const float* feat,
+                                                   const int32_t* __restrict__ lo2gid, const float* D, const float* Hp, int vw, const float* Wa,
+                                                   const int32_t* __restrict__ irp, const int32_t* __restrict__ icol, const float* a,
+                                                   const int32_t* __restrict__ pi, const int32_t* __restrict__ pj, const int32_t* __restrict__ ppij,
+                                                   const int32_t* __restrict__ ppji, const float* P, float* t, float* cw, float* dHa, float* gFw,
+                                                   float* zs, int tid, int nt, int warp, int nwarps, int lane) {
+  const int dp = gx_round_up(d, 4);
+  for (int i = warp; i < nrow; i += nwarps) {
+    const float* const Di = D + (int64_t)i * (Hp == nullptr ? dp : vw);
+    for (int e = irp[i] + lane; e < irp[i + 1]; e += 32) {
+      const int j = icol[e];
+      float tv = 0.f;
+      if (Hp == nullptr) {
+        const float* const x = feat + (int64_t)lo2gid[j] * d;
+        for (int f = 0; f < d; ++f) tv = fmaf(Di[f], __ldg(x + f), tv);
+      } else {
+        const float* const h = Hp + (int64_t)j * vw;
+        for (int f = 0; f < win; ++f) tv = fmaf(Di[f], h[f], tv);
+      }
+      t[e] = tv;
+    }
+  }
+  __syncthreads();
+  for (int p = tid; p < np; p += nt) {
+    const int i = pi[p], j = pj[p];
+    const float tij = i < nrow ? t[ppij[p]] : 0.f, tji = j < nrow ? t[ppji[p]] : 0.f;
+    const float c = (i < nsrows ? a[ppij[p]] : a[ppji[p]]) * (tij + tji);
+    cw[ppij[p]] = c;
+    cw[ppji[p]] = c;
+  }
+  __syncthreads();
+  for (int i = warp; i < nin; i += nwarps) {
+    const int r0 = irp[i], r1 = irp[i + 1];
+    for (int c0 = 0; c0 < win; c0 += 32) {
+      const int c = c0 + lane;
+      float v = 0.f;
+      if (c < win)
+        for (int e = r0; e < r1; ++e) {
+          const int j = icol[e];
+          if (i >= nrow && j >= nrow) break;   // columns are partitioned by level
+          v = fmaf(cw[e], P[(int64_t)j * ldp + c], v);
+        }
+      if (c < win) zs[c] = v;
+    }
+    __syncwarp();
+    // [dL/dP_i Wa^T]_f = sum_c dL/dP_i[c] Wa[f][c]: lanes over c (consecutive words of Wa's row f), one warp sum per f; lane f % 32
+    // owns entry f, as in the row phase
+    const float* const x = Hp == nullptr ? feat + (int64_t)lo2gid[i] * d : nullptr;
+    for (int f = 0; f < win; ++f) {
+      float q = 0.f;
+      for (int c = lane; c < win; c += 32) q = fmaf(zs[c], Wa[f * win + c], q);
+      q = warp_sum(q);
+      if (lane == (f & 31)) {
+        if (Hp == nullptr) gFw[f] = fmaf(q, __ldg(x + f), gFw[f]);
+        else dHa[(int64_t)i * vw + f] = q;
+      }
+    }
+    __syncwarp();
+  }
+  __syncthreads();
+}
+
 // The minimum-blocks bound 0 is the compiler's default: node mode is capped at 128 registers (some instantiations spill); graph mode
 // lets the small default-width model fit two CTAs per SM.
-template <bool kGraph, bool kBn, int KW>
+template <bool kGraph, bool kBn, int KW, bool kAtt>
 __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1) : 0) explain_var_kernel(const VarArgs A) {
   extern __shared__ __align__(16) float sm[];
   __shared__ int s_task;
@@ -56,7 +171,7 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
   const int dp = gx_round_up(d, 4);
   const int PD = hid * (L - 1) + embw;
   const bool ieee = (hp.flags & GX_HP_IEEE_EDGE) != 0;
-  const VarSmem S = var_smem(d, L, hid, embw, C, nwarps);
+  const VarSmem S = var_smem(d, L, hid, embw, C, nwarps, kAtt ? 1 : 0);
   float* const sF = sm + S.sF; float* const Fm = sm + S.F; float* const mF = sm + S.mF; float* const vF = sm + S.vF;
   float* const zs = sm + S.zs + warp * S.zlen;
   float* const gFp = sm + S.gFp;
@@ -71,6 +186,8 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
 
   const float* Wl[GX_MAX_LAYERS];   // conv weights: shared memory when they fit, else global (L2 resident)
   var_stage_model(m, S, sm, Wl, tid, NT);
+  const float* Wal[kAtt ? GX_MAX_LAYERS : 1];  // attention weights (kAtt), staged like Wl
+  if constexpr (kAtt) var_stage_att(m, S, sm, Wal, tid, NT);
   if constexpr (kGraph) {
     __syncthreads();
     // embedding of a row without edges: Y = 0 W + b, the same activation as any row; depends on the model only
@@ -103,7 +220,8 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
       for (int l = 1; l <= L; ++l) R[l] = Tp->cum[L - l] < n ? Tp->cum[L - l] : n;
     }
     auto rows = [&](int l) { if constexpr (kGraph) return n; else return R[l]; };
-    const GxVarLayout Lo = gx_make_var_layout(n, n2, e1, kGraph ? 0 : np, d, L, VW);
+    auto rin = [&](int l) { if constexpr (kGraph) return n; else return R[l - 1]; };   // input rows of layer l
+    const GxVarLayout Lo = gx_make_var_layout(n, n2, e1, kGraph ? 0 : np, d, L, VW, kAtt ? 1 : 0, Tp->e_d);
     // layer 1's input rows: the graph's features (node mode), this graph's padded rows (graph mode); both indexed by lo2gid
     const float* const feat = kGraph ? A.gb.feat + (int64_t)Tp->node * A.gb.max_nodes * d : A.g.feat;
     const int32_t* __restrict__ lo2gid = A.plan.lo2gid + node_off;
@@ -118,6 +236,12 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
     auto dZ = [&](int l) { return slab + Lo.dZ + (int64_t)(l - 2) * n2 * VW; };     // l = 2..L: dL/d(A_m H_{l-1}) (width hid)
     auto qn = [&](int l) { return slab + Lo.q + (int64_t)(l - 1) * n2; };
     auto istd = [&](int l) { return slab + Lo.istd + (int64_t)(l - 1) * n2; };
+    // attention (kAtt): P of layer l (row stride dp on layer 1, VW above), per-slot s, a s and t of layer l
+    auto Pl = [&](int l) { return slab + Lo.P + (l == 1 ? 0 : (int64_t)n * dp + (int64_t)(l - 2) * n2 * VW); };
+    auto sl = [&](int l) { return slab + Lo.s + (int64_t)(l - 1) * e1; };
+    auto asl = [&](int l) { return slab + Lo.as + (int64_t)(l - 1) * e1; };
+    auto tl = [&](int l) { return slab + Lo.t + (int64_t)(l - 1) * e1; };
+    float* const cw = slab + Lo.cw; float* const dHa = slab + Lo.dHa;
     float2* const mm = MM + np; float2* const vv = mm + np; float2* const SS = vv + np;
     const float nn = (float)Tp->n_norm * (float)Tp->n_norm;
     const float ent_over_nn = hp.c_ent / nn;
@@ -156,10 +280,16 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
       for (int l = 1; l <= L; ++l) {
         const int win = win_of(l - 1), wout = wout_of(l - 1);
         const float* const Ws = Wl[l - 1]; const float* const bsm = sm + S.b[l - 1];
+        const float* ag = a;   // the aggregation weights: a, or a s on attention models
+        if constexpr (kAtt) {
+          att_forward_edges(win, l == 1 ? dp : VW, rin(l), kGraph ? n : n2, d, feat, lo2gid, sF, l == 1 ? nullptr : Hh(l - 1), VW,
+                            Wal[l - 1], irp, icol, a, Pl(l), sl(l), asl(l), zs, warp, nwarps, lane);
+          ag = asl(l);
+        }
         for (int i = warp; i < rows(l); i += nwarps) {
           const int r0 = irp[i], r1 = irp[i + 1];
-          if (l == 1) var_gather_feat(r0, r1, icol, a, feat, lo2gid, d, sF, U + (int64_t)i * dp, zs, lane);
-          else var_gather_hidden<KW>(r0, r1, icol, a, Hh(l - 1), win, zs, lane);
+          if (l == 1) var_gather_feat(r0, r1, icol, ag, feat, lo2gid, d, sF, U + (int64_t)i * dp, zs, lane);
+          else var_gather_hidden<KW>(r0, r1, icol, ag, Hh(l - 1), win, zs, lane);
           var_row_forward<kBn, KW>(zs, win, Ws, wout, bsm, l, L, i, Yh, Hh, VW, qn, istd, lane);
         }
         __syncthreads();
@@ -189,7 +319,12 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
           float g[KW], yh[KW];
 #pragma unroll
           for (int k = 0; k < KW; ++k) g[k] = 0.f;
-          if (l < L) var_gather_back<KW>(irp[i], irp[i + 1], icol, a, dZ(l + 1), wout, rows(l + 1), g, lane);   // columns are partitioned by level
+          if (l < L) var_gather_back<KW>(irp[i], irp[i + 1], icol, kAtt ? asl(l + 1) : a, dZ(l + 1), wout, rows(l + 1), g, lane);   // columns are partitioned by level
+          if constexpr (kAtt) {   // + the attention's share, dL/dP_{l+1} Wa_{l+1}^T
+#pragma unroll
+            for (int k = 0; k < KW; ++k)
+              if (l < L && lane + 32 * k < wout) g[k] += dHa[(int64_t)i * VW + lane + 32 * k];
+          }
 #pragma unroll
           for (int k = 0; k < KW; ++k) {
             const int c = lane + 32 * k;
@@ -203,6 +338,10 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
           __syncwarp();
         }
         __syncthreads();
+        if constexpr (kAtt)
+          att_backward_edges(win, l == 1 ? dp : VW, rows(l), rin(l), kGraph ? n : n2, np, d, feat, lo2gid, l == 1 ? dZ1 : dZ(l),
+                             l == 1 ? nullptr : Hh(l - 1), VW, Wal[l - 1], irp, icol, a, pi, pj, ppij, ppji, Pl(l), tl(l), cw, dHa,
+                             gFp + warp * dp, zs, tid, NT, warp, nwarps, lane);
       }
       // ---------------------------------------------------------------- P: edge gradients, regularisers, optimiser step, next mask
       {
@@ -225,7 +364,15 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
           const int i = pi[p], j = pj[p];   // i < j in level order
           // dL/dA_ij + dL/dA_ji = sum over the layers of <dL/d(A_m H_{l-1})[i], H_{l-1}[j]> + <.. [j], .. [i]> (layer 1: feature rows)
           float Gd;
-          if constexpr (kGraph) {   // no Laplacian term; every row at every layer, both directions of a layer in one sum
+          if constexpr (kAtt) {   // sum over the layers of s_ij (t_ij + t_ji), t of the rows of the layer only
+            Gd = kGraph ? 0.f : lapg[p];
+            for (int l = 1; l <= L; ++l) {
+              const bool ri = kGraph || i < R[l], rj = kGraph || j < R[l];
+              if (!ri && !rj) continue;
+              const float tij = ri ? tl(l)[ppij[p]] : 0.f, tji = rj ? tl(l)[ppji[p]] : 0.f;
+              Gd = fmaf(sl(l)[ppij[p]], tij + tji, Gd);
+            }
+          } else if constexpr (kGraph) {   // no Laplacian term; every row at every layer, both directions of a layer in one sum
             Gd = 0.f;
             {
               const float* xi = feat + (int64_t)lo2gid[i] * d; const float* xj = feat + (int64_t)lo2gid[j] * d;
@@ -286,22 +433,24 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
 template <typename F>
 cudaError_t with_var_kernel(int graph_mode, const GxModelDev& m, F&& f) {
   return var_dispatch(m, [&](auto bn, auto kw) {
-    return graph_mode ? f(explain_var_kernel<true, decltype(bn)::value, decltype(kw)::value>)
-                      : f(explain_var_kernel<false, decltype(bn)::value, decltype(kw)::value>);
+    constexpr bool b = decltype(bn)::value;
+    constexpr int w = decltype(kw)::value;
+    if (m.att) return graph_mode ? f(explain_var_kernel<true, b, w, true>) : f(explain_var_kernel<false, b, w, true>);
+    return graph_mode ? f(explain_var_kernel<true, b, w, false>) : f(explain_var_kernel<false, b, w, false>);
   });
 }
 
 }  // namespace
 
 // var_smem's carve-up + in graph mode the edge-less rows' constant embedding and the arg-max row of every pooled feature (cst, arg)
-int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C) {
+int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C, int att) {
   const int pool = graph_mode ? 2 * gx_round_up(hid * (L - 1) + emb, 4) : 0;
-  return (var_smem(d, L, hid, emb, C, kVarThreads / 32).total + pool) * 4;
+  return (var_smem(d, L, hid, emb, C, kVarThreads / 32, att).total + pool) * 4;
 }
 int gx_var_row_stride(int hid, int emb) { return 32 * var_kw(hid, emb); }
 
 int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m) {
-  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C);
+  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C, m.att);
   int n = 0;
   with_var_kernel(graph_mode, m, [&](auto kern) { n = var_ctas_per_sm(kern, bytes); return cudaSuccess; });
   return n;
@@ -313,6 +462,6 @@ cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, int graph_mode, co
   VarArgs args;
   fill_queue_args(args, cfg, m, hp, plan, m0, out_mask, out_feat);
   args.g = g; args.gb = gb; args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
-  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C);
+  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C, m.att);
   return with_var_kernel(graph_mode, m, [&](auto kern) { return var_launch(kern, args, cfg.grid, bytes, s); });
 }

@@ -16,9 +16,24 @@ constexpr int kVarWeightWords = 36 * 1024;   // conv weights are staged in share
 __host__ __device__ inline int var_kw(int hid, int emb) { const int w = hid > emb ? hid : emb; return w <= 32 ? 1 : (w <= 64 ? 2 : 4); }
 
 // Shared-memory carve-up (words) of the model-variant kernels: conv weights (when they fit) and biases, pred_model, the feature-mask
-// state, per-warp scratch rows and partial dL/dsF, the readout vectors.
+// state, per-warp scratch rows and partial dL/dsF, the readout vectors.  Attention models (att != 0) also stage the (in, in)
+// attention weights when they fit the weight budget together with the conv weights (var_att_in_smem): the last var_att_words words
+// before S.total, layer by layer; else they are read through L2 and the conv weights are staged as for any other model.
 struct VarSmem { int W[GX_MAX_LAYERS], b[GX_MAX_LAYERS], Wp, sF, F, mF, vF, zs, zlen, gFp, emb, dEmb, logit, w_in_smem, total; };
-__host__ __device__ inline VarSmem var_smem(int d, int L, int hid, int emb, int C, int nwarps) {
+__host__ __device__ inline int var_att_words(int d, int L, int hid) {
+  int w = 0;
+  for (int l = 0; l < L; ++l) w += gx_round_up((l == 0 ? d : hid) * (l == 0 ? d : hid), 4);
+  return w;
+}
+__host__ __device__ inline int var_conv_words(int d, int L, int hid, int emb) {
+  int w = 0;
+  for (int l = 0; l < L; ++l) w += (l == 0 ? d : hid) * (l == L - 1 ? emb : hid);
+  return w;
+}
+__host__ __device__ inline bool var_att_in_smem(int d, int L, int hid, int emb) {
+  return var_conv_words(d, L, hid, emb) + var_att_words(d, L, hid) <= kVarWeightWords;
+}
+__host__ __device__ inline VarSmem var_smem(int d, int L, int hid, int emb, int C, int nwarps, int att = 0) {
   VarSmem S;
   const int dp = gx_round_up(d, 4);
   int o = 0;
@@ -38,6 +53,7 @@ __host__ __device__ inline VarSmem var_smem(int d, int L, int hid, int emb, int 
   S.zs = take(nwarps * S.zlen);
   S.gFp = take(nwarps * dp);
   S.emb = take(PD); S.dEmb = take(PD); S.logit = take(C < 32 ? 32 : C);
+  if (att && var_att_in_smem(d, L, hid, emb)) take(var_att_words(d, L, hid));
   S.total = o;
   return S;
 }
@@ -57,6 +73,18 @@ __device__ __forceinline__ void var_stage_model(const GxModelDev& m, const VarSm
   if (m.C * (PD + 1) <= GX_WP_SMEM_MAX) {
     for (int idx = tid; idx < m.C * PD; idx += nt) sm[S.Wp + idx] = __ldg(m.Wp + idx);
     for (int idx = tid; idx < m.C; idx += nt) sm[S.Wp + m.C * PD + idx] = __ldg(m.bp + idx);
+  }
+}
+// Attention models: stages the attention weights when var_att_in_smem; Wal[l] = where layer l's are read from.
+__device__ __forceinline__ void var_stage_att(const GxModelDev& m, const VarSmem& S, float* sm, const float** Wal, int tid, int nt) {
+  const bool in_smem = var_att_in_smem(m.d, m.L, m.hid, m.emb);
+  int o = S.total - var_att_words(m.d, m.L, m.hid);
+  for (int l = 0; l < m.L; ++l) {
+    const int win = l == 0 ? m.d : m.hid;
+    if (in_smem)
+      for (int idx = tid; idx < win * win; idx += nt) sm[o + idx] = __ldg(gx_att_weight(m, l) + idx);
+    Wal[l] = in_smem ? sm + o : gx_att_weight(m, l);
+    o += gx_round_up(win * win, 4);
   }
 }
 

@@ -3,7 +3,8 @@
 // from the checkpoint; `Explainer(pred=None)` computes it here).  Unmasked adjacency, no feature mask, any num_layers <= 4, --bn.
 // One launch per layer (a layer reads every row of the previous one), a warp per node with lane = feature -- the same row
 // arithmetic as explain_var.cu: Y = (sum_{j in N(i)} H_{l-1}[j]) W_l + b_l, row L2-normalise, ReLU (+ per-node standardisation
-// with --bn) on hidden layers; logits = pred_model(concat of the layer outputs).
+// with --bn) on hidden layers; logits = pred_model(concat of the layer outputs).  Attention models (--method att, models.py:62-68) first
+// project P = H_{l-1} Wa_l (att_project_kernel) and weight every edge, self loops included, by s_ij = P_i . P_j.
 #include <algorithm>
 
 #include "explain_common.cuh"
@@ -12,11 +13,38 @@ namespace {
 
 constexpr int kFwdThreads = 256;
 
+// P = Hin Wa for all N nodes (attention models): a warp per node, Hin rows of stride ldin, P rows of stride ldp = round_up(win, 4)
+__global__ void __launch_bounds__(kFwdThreads) att_project_kernel(int64_t N, const float* __restrict__ Hin, int ldin, const float* __restrict__ Wa, int win,
+                                                                  float* __restrict__ P) {
+  extern __shared__ float zs_all[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = kFwdThreads / 32;
+  const int ldp = gx_round_up(win, 4);
+  float* const zs = zs_all + warp * ldp;
+  for (int64_t i = (int64_t)blockIdx.x * nwarps + warp; i < N; i += (int64_t)gridDim.x * nwarps) {
+    for (int f = lane; f < win; f += 32) zs[f] = Hin[i * ldin + f];
+    __syncwarp();
+    for (int c = lane; c < win; c += 32) {
+      float p = 0.f;
+      for (int f = 0; f < win; ++f) p = fmaf(zs[f], __ldg(Wa + f * win + c), p);
+      P[i * ldp + c] = p;
+    }
+    __syncwarp();
+  }
+}
+
+// s_ij = P_i . P_j (every lane gets it); P rows of stride round_up(win, 4)
+__device__ __forceinline__ float att_score(const float* __restrict__ P, int64_t i, int64_t j, int win, int lane) {
+  const int ldp = gx_round_up(win, 4);
+  float sp = 0.f;
+  for (int f = lane; f < win; f += 32) sp = fmaf(P[i * ldp + f], P[j * ldp + f], sp);
+  return warp_sum(sp);
+}
+
 // one GCN layer for all N nodes.  Hin: [N][32] (layer > 1) or the feature matrix [N][d] (layer 1); Hout: [N][32] what the next layer /
-// the readout sees (relu / standardised on hidden layers, the normalised output on the last).
-template <bool kFirst>
+// the readout sees (relu / standardised on hidden layers, the normalised output on the last).  kAtt: edge weights s_ij from P.
+template <bool kFirst, bool kAtt>
 __global__ void __launch_bounds__(kFwdThreads) gcn_layer_kernel(GxGraphDev g, const float* __restrict__ Hin, const float* __restrict__ W, const float* __restrict__ b,
-                                                                int win, int wout, int last, int bn, float* __restrict__ Hout) {
+                                                                int win, int wout, int last, int bn, const float* __restrict__ P, float* __restrict__ Hout) {
   extern __shared__ float zs_all[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = kFwdThreads / 32;
   const int dp = gx_round_up(win, 4);
@@ -24,7 +52,22 @@ __global__ void __launch_bounds__(kFwdThreads) gcn_layer_kernel(GxGraphDev g, co
   for (int64_t i = (int64_t)blockIdx.x * nwarps + warp; i < g.N; i += (int64_t)gridDim.x * nwarps) {
     const int r0 = g.rowptr[i], r1 = g.rowptr[i + 1];
     float y = lane < wout ? __ldg(b + lane) : 0.f;
-    if (kFirst) {
+    if constexpr (kAtt) {   // zs = (A (.) s) Hin[i]: every lane takes part in every edge's score
+      for (int f0 = 0; f0 < win; f0 += 32) {
+        const int f = f0 + lane;
+        float z = 0.f;
+        for (int e = r0; e < r1; ++e) {
+          const int64_t j = g.col[e];
+          const float se = att_score(P, i, j, win, lane);
+          if (f < win) z = fmaf(se, Hin[j * (kFirst ? win : 32) + f], z);
+        }
+        if (f < win) zs[f] = z;
+      }
+      __syncwarp();
+      if (lane < wout)
+        for (int f = 0; f < win; ++f) y = fmaf(zs[f], __ldg(W + f * wout + lane), y);
+      __syncwarp();
+    } else if (kFirst) {
       for (int f0 = 0; f0 < win; f0 += 32) {
         const int f = f0 + lane;
         float z = 0.f;
@@ -86,8 +129,9 @@ __global__ void __launch_bounds__(kFwdThreads) readout_kernel(int64_t N, int L, 
 
 }  // namespace
 
-// H: workspace [L][N][32] floats (device).  pred [N][C], emb_out [N][PD] or nullptr (device).
-cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, float* pred, float* emb_out, cudaStream_t s) {
+// H: workspace [L][N][32] floats (device).  pred [N][C], emb_out [N][PD] or nullptr (device).  P: attention models' workspace
+// [N][round_up(max(d, hid), 4)] floats (device), else unused.
+cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, float* pred, float* emb_out, float* P, cudaStream_t s) {
   const int nwarps = kFwdThreads / 32;
   const int grid = (int)std::min<int64_t>((g.N + nwarps - 1) / nwarps, GX_GRID_CAP);
   for (int l = 0; l < m.L; ++l) {
@@ -95,8 +139,14 @@ cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, fl
     const float* Hin = l == 0 ? g.feat : H + (int64_t)(l - 1) * g.N * 32;
     float* Hout = H + (int64_t)l * g.N * 32;
     const size_t smem = (size_t)nwarps * gx_round_up(win, 4) * sizeof(float);
-    if (l == 0) gcn_layer_kernel<true><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, Hout);
-    else gcn_layer_kernel<false><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, Hout);
+    if (m.att) {
+      att_project_kernel<<<grid, kFwdThreads, smem, s>>>(g.N, Hin, l == 0 ? win : 32, gx_att_weight(m, l), win, P);
+      if (l == 0) gcn_layer_kernel<true, true><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, P, Hout);
+      else gcn_layer_kernel<false, true><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, P, Hout);
+      continue;
+    }
+    if (l == 0) gcn_layer_kernel<true, false><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, nullptr, Hout);
+    else gcn_layer_kernel<false, false><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, nullptr, Hout);
   }
   readout_kernel<<<grid, kFwdThreads, 0, s>>>(g.N, m.L, m.hid, m.emb, m.C, H, m.Wp, m.bp, pred, emb_out);
   return cudaGetLastError();

@@ -69,13 +69,19 @@ struct GxGraphDev {
 struct GxModelDev {
   int32_t d, hid, emb, C, L;
   int32_t bn;          // --bn: per-node standardisation after every hidden ReLU (models.py:222-228)
-  int32_t variant;     // 1: num_layers != 3 or bn -> every task runs in explain_var.cu with the UNPADDED widths hid / emb
+  int32_t variant;     // 1: num_layers != 3 or bn or att -> every task runs in explain_var.cu with the UNPADDED widths hid / emb
+  int32_t att;         // --method att: every layer scales the masked adjacency by s_ij = P_i . P_j, P = H_{l-1} Wa_l (models.py:62-68)
   const float* W[GX_MAX_LAYERS];   // row-major (in,out)
   const float* Wt[GX_MAX_LAYERS];  // row-major (out,in) (default model only)
   const float* b[GX_MAX_LAYERS];   // never NULL on device (zeros when --nobias)
   const float* Wp;     // (C, 2*hid+emb)
   const float* bp;
 };
+// att models: layer l's attention weights (conv_*.att_weight, row-major (in, in)) follow its conv weights in the model buffer, so the
+// struct (a kernel argument of every explainer kernel) keeps its size
+__host__ __device__ inline const float* gx_att_weight(const GxModelDev& m, int l) {
+  return m.W[l] + (l == 0 ? m.d : m.hid) * (l == m.L - 1 ? m.emb : m.hid);
+}
 
 struct GxHparamsDev {
   int32_t iters;     // forward/backward/update iterations executed: num_epochs - 1 (the last epoch's backward is unobservable), num_epochs when a trace is requested
@@ -202,11 +208,15 @@ __host__ __device__ inline GxStreamLayout gx_make_stream_layout(int n, int n1, i
 
 // Global-memory slab of one task in the model-variant kernel (explain_var.cu); hidden-width arrays have row stride vw = 32 * ceil(width / 32).
 // Graph mode computes every one of its n rows with an edge at every layer (n2 = n, e1 = e_d) and has no Laplacian term (np_in = 0).
+// Attention models (att != 0, e_d = all directed slots of the task) add the per-layer projections and edge weights; for any other
+// model these arrays take zero words.
 struct GxVarLayout {
   int64_t a, U, dZ1, lapg, Yh, H, dZ, q, istd;
+  int64_t P, s, as, t, cw, dHa;
   int64_t total_words;
 };
-__host__ __device__ inline GxVarLayout gx_make_var_layout(int n, int n2, int e1, int np_in, int d, int L, int vw = 32) {
+__host__ __device__ inline GxVarLayout gx_make_var_layout(int n, int n2, int e1, int np_in, int d, int L, int vw = 32, int att = 0,
+                                                          int e_d = 0) {
   GxVarLayout Lo;
   const int dp = gx_round_up(d, 4);
   int64_t o = 0;
@@ -221,6 +231,13 @@ __host__ __device__ inline GxVarLayout gx_make_var_layout(int n, int n2, int e1,
   Lo.dZ = take((int64_t)(L - 1) * n2 * vw);   // layers 2..L: dL/d(A_m H_{l-1})
   Lo.q = take((int64_t)L * n2);
   Lo.istd = take((int64_t)L * n2);
+  const int64_t at = att ? 1 : 0;
+  Lo.P = take(at * ((int64_t)n * dp + (int64_t)(L - 1) * n2 * vw));   // per layer: P = H_{l-1} Wa on the layer's input rows (layer 1: n rows, stride dp)
+  Lo.s = take(at * L * e1);                   // per layer and slot: s_ij = P_i . P_j
+  Lo.as = take(at * L * e1);                  // per layer and slot: the aggregation weight a_ij s_ij
+  Lo.t = take(at * L * e1);                   // per layer and slot of a row of the layer: t_ij = dL/dZ_i . H_{l-1}[j]
+  Lo.cw = take(at * e_d);                     // the current layer's a_ij (t_ij + t_ji) on every slot (rows beyond n2 included)
+  Lo.dHa = take(at * n2 * vw);                // dL/dP Wa^T of the layer above: the attention's share of dL/dH
   Lo.total_words = o;
   return Lo;
 }
@@ -355,7 +372,7 @@ cudaError_t gx_launch_explain_gang(const GxExplainLaunch& cfg, const GxGraphDev&
                                    const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                    float* out_mask, float* out_feat, cudaStream_t s);
 int gx_gang_smem_bytes(int d, int hid, int C);
-cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, float* pred, float* emb_out, cudaStream_t s);
+cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, float* pred, float* emb_out, float* P, cudaStream_t s);
 constexpr int GX_STREAM_THREADS = 768;  // 24 warps: 80 registers per thread, 5 KB of cp.async staging per warp
 int gx_explain_max_smem();
 struct GxGraphBatchDev {
@@ -373,7 +390,7 @@ cudaError_t gx_launch_explain_graphs(const GxExplainLaunch& cfg, const GxGraphBa
 cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
                                   const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                   float* out_mask, float* out_feat, cudaStream_t s);
-int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C);
+int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C, int att = 0);
 int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m);
 int gx_var_row_stride(int hid, int emb);
 // explain_dense.cu: Explainer.explain(..., unconstrained=True), node mode (graph_mode 0, g) or graph mode (gb); m0 / out_dense are dense

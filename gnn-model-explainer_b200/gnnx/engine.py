@@ -103,9 +103,10 @@ class Engine:
     def sync(self):
         _abi.check(self._lib.gx_sync(self._h))
 
-    def set_model(self, weights, num_layers=3, bn=False):
+    def set_model(self, weights, num_layers=3, bn=False, att=None):
         """weights: dict W1,b1,W2,b2,W3,b3,Wp,bp (numpy; b* may be None).  Shapes are checked here: the C ABI takes bare
-        pointers, so a checkpoint whose layers do not chain (or a concat=False / MLP prediction head) must not reach it."""
+        pointers, so a checkpoint whose layers do not chain (or a concat=False / MLP prediction head) must not reach it.
+        att: an attention model's (in, in) conv_*.att_weight matrices, one per layer (gx_set_model_att); None for any other model."""
         Ws = [_f32c(weights["W%d" % (l + 1)]) for l in range(num_layers)]
         bs = [None if weights.get("b%d" % (l + 1)) is None else _f32c(weights["b%d" % (l + 1)])
               for l in range(num_layers)]
@@ -128,11 +129,23 @@ class Engine:
             raise ValueError("pred_model.weight is %s, expected (C, %d) = concat of the layer outputs" % (Wp.shape, pd))
         if bp.shape != (Wp.shape[0],):
             raise ValueError("pred_model.bias is %s, expected (%d,)" % (bp.shape, Wp.shape[0]))
-        dims = _abi.GxModelDims(Ws[0].shape[0], Ws[0].shape[1], Ws[-1].shape[1], Wp.shape[0], num_layers,
-                                _abi.GX_MODEL_BN if bn else 0)
         wp = (C.c_void_p * num_layers)(*[w.ctypes.data for w in Ws])
         bp_arr = (C.c_void_p * num_layers)(*[(b.ctypes.data if b is not None else None) for b in bs])
-        _abi.check(self._lib.gx_set_model(self._h, C.byref(dims), wp, bp_arr, _np_ptr(Wp), _np_ptr(bp)))
+        if att is None:
+            dims = _abi.GxModelDims(Ws[0].shape[0], Ws[0].shape[1], Ws[-1].shape[1], Wp.shape[0], num_layers,
+                                    _abi.GX_MODEL_BN if bn else 0)
+            _abi.check(self._lib.gx_set_model(self._h, C.byref(dims), wp, bp_arr, _np_ptr(Wp), _np_ptr(bp)))
+        else:
+            Was = [_f32c(a) for a in att]
+            if len(Was) != num_layers:
+                raise ValueError("att: %d attention matrices for %d layers" % (len(Was), num_layers))
+            for l, a in enumerate(Was):
+                if a.shape != (Ws[l].shape[0], Ws[l].shape[0]):
+                    raise ValueError("layer %d att_weight is %s, expected (%d, %d)" % (l + 1, a.shape, Ws[l].shape[0], Ws[l].shape[0]))
+            dims = _abi.GxModelDims(Ws[0].shape[0], Ws[0].shape[1], Ws[-1].shape[1], Wp.shape[0], num_layers,
+                                    (_abi.GX_MODEL_BN if bn else 0) | _abi.GX_MODEL_ATT)
+            ap = (C.c_void_p * num_layers)(*[a.ctypes.data for a in Was])
+            _abi.check(self._lib.gx_set_model_att(self._h, C.byref(dims), wp, bp_arr, ap, _np_ptr(Wp), _np_ptr(bp)))
         self.input_dim = int(Ws[0].shape[0])
         self.num_classes = int(Wp.shape[0])
 

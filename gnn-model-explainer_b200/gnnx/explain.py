@@ -52,7 +52,7 @@ def gen_explainer_prefix(args):
 def model_weights(model):
     """state_dict of a reference (or gnnx) GcnEncoderNode/GcnEncoderGraph -> weight dict.
     Keys as in the reference checkpoints (SURVEY 8a8): conv_first / conv_block.i / conv_last /
-    pred_model."""
+    pred_model; an attention model (--method att) also has <layer>.att_weight, returned as Wa1 .. WaL."""
     sd = {k: v.detach().cpu().float().numpy() for k, v in model.state_dict().items()}
     if "pred_model.weight" not in sd:
         raise NotImplementedError("pred_hidden_dims != [] (MLP prediction head) is not built")
@@ -64,8 +64,12 @@ def model_weights(model):
     for l, nm in enumerate(names, 1):
         w["W%d" % l] = sd[nm + ".weight"]
         w["b%d" % l] = sd.get(nm + ".bias")
-        if (nm + ".self_weight") in sd or (nm + ".att_weight") in sd:
-            raise NotImplementedError("add_self / att GraphConv variants are out of scope")
+        if (nm + ".self_weight") in sd:
+            raise NotImplementedError("the add_self GraphConv variant is out of scope")
+        if (nm + ".att_weight") in sd:
+            w["Wa%d" % l] = sd[nm + ".att_weight"]
+    if any(("Wa%d" % l) in w for l in range(1, len(names) + 1)) and not all(("Wa%d" % l) in w for l in range(1, len(names) + 1)):
+        raise ValueError("att_weight on some conv layers only")
     w["Wp"], w["bp"] = sd["pred_model.weight"], sd["pred_model.bias"]
     return w, len(names)
 
@@ -101,11 +105,13 @@ class Explainer:
             device = int(os.environ.get("LOCAL_RANK", "0")) if torch.cuda.is_available() else 0
         self.engine = Engine(device)
         weights, num_layers = model_weights(model)
-        self.engine.set_model(weights, num_layers=num_layers, bn=bn)
+        self._att = "Wa1" in weights
+        self.engine.set_model(weights, num_layers=num_layers, bn=bn,
+                              att=[weights["Wa%d" % l] for l in range(1, num_layers + 1)] if self._att else None)
         if getattr(args, "gnnx_latency", False):
             self.engine.debug_cluster(0, 0)   # latency mode: thread-block clusters for the expensive tasks of batches that leave SMs idle
         # model / optimiser variants run in the variant kernel, which does not log the per-epoch trace print_training replays
-        self._no_trace = bn or num_layers != 3 or getattr(args, "opt", "adam") != "adam"
+        self._no_trace = bn or num_layers != 3 or getattr(args, "opt", "adam") != "adam" or self._att
         adj_np = np.asarray(adj)
         if graph_mode:
             # graph classification: the whole padded batch goes to the device once (explain.py:80-85)
@@ -239,6 +245,8 @@ class Explainer:
                 self._draw_m0(plan)
             self.engine.grad_nodes_host(edge_mask)     # (unconstrained is ignored here, as in the reference)
             return plan, edge_mask
+        if unconstrained and self._att:
+            raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
         hp, init = self._hparams()
         if unconstrained:
             # explain.py:688-692: the dense mask drives the forward, so every one of the n^2 normals of M0 is a parameter
@@ -253,7 +261,7 @@ class Explainer:
             return plan, edge_mask
         if not self.print_training or self._no_trace:
             if self.print_training:
-                print("(per-epoch trace is not built for --bn / num_gc_layers != 3 / optimisers other than Adam)")
+                self._print_no_trace()
             m0 = self._draw_m0(plan) if init == "torch" else None
             self.engine.explain_nodes_host(hp, m0, edge_mask)
             return plan, edge_mask
@@ -265,6 +273,12 @@ class Explainer:
         off = self.engine.offedge_regularisers(hp, np.concatenate([D.reshape(-1) for D in dense])) if dense is not None else None
         self.last_trace = self._print_trace(plan, hp, trace, pred, off)
         return plan, edge_mask
+
+    def _print_no_trace(self):
+        if self._att:
+            print("(per-epoch trace is not built for attention models (--method att))")
+        else:
+            print("(per-epoch trace is not built for --bn / num_gc_layers != 3 / optimisers other than Adam)")
 
     def _print_trace(self, plan, hp, trace, pred, off):
         """Replays the reference's per-epoch print (explain.py:148-159).  With the torch-compatible init the loss is the
@@ -292,11 +306,13 @@ class Explainer:
 
     # ---------------------------------------------------------------- public API
     def _explain_graph_batch(self, graph_indices, unconstrained=False):
+        if unconstrained and self._att:
+            raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
         gids = [int(g) for g in graph_indices]
         edge_off = self.engine.plan_graphs(gids)
         hp, init = self._hparams()
         if self.print_training and self._no_trace and not unconstrained:
-            print("(per-epoch trace is not built for --bn / num_gc_layers != 3 / optimisers other than Adam)")
+            self._print_no_trace()
         n = self.engine.batch_n
         m0 = None
         rc = [self.engine.graph_rows_cols(g) for g in gids]

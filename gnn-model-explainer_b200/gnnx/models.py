@@ -14,13 +14,14 @@ from torch.nn import init
 
 
 class GraphConv(nn.Module):
-    """models.py:9-80.  y = normalize((adj @ x) @ W + b); att / add_self variants are out of scope."""
+    """models.py:9-80.  y = normalize((adj @ x) @ W + b); with att, adj is first scaled by the unnormalised attention
+    (x Wa)(x Wa)^T (models.py:62-68).  The add_self variant is out of scope."""
 
     def __init__(self, input_dim, output_dim, add_self=False, normalize_embedding=False, dropout=0.0,
                  bias=True, gpu=True, att=False):
         super().__init__()
-        if att or add_self:
-            raise NotImplementedError("att / add_self GraphConv variants are out of scope (SURVEY 8f)")
+        if add_self:
+            raise NotImplementedError("the add_self GraphConv variant is out of scope (SURVEY 8f)")
         self.att = att
         self.add_self = add_self
         self.dropout = dropout
@@ -30,11 +31,16 @@ class GraphConv(nn.Module):
         self.input_dim = input_dim
         self.output_dim = output_dim
         self.weight = nn.Parameter(torch.empty(input_dim, output_dim))
+        if att:
+            self.att_weight = nn.Parameter(torch.empty(input_dim, input_dim))
         self.bias = nn.Parameter(torch.empty(output_dim)) if bias else None
 
     def forward(self, x, adj):
         if self.dropout > 0.001:
             x = self.dropout_layer(x)
+        if self.att:
+            x_att = torch.matmul(x, self.att_weight)
+            adj = adj * (x_att @ x_att.permute(0, 2, 1))
         y = torch.matmul(torch.matmul(adj, x), self.weight)
         if self.bias is not None:
             y = y + self.bias
@@ -58,12 +64,10 @@ class GcnEncoderGraph(nn.Module):
         self.bias = True if args is None else getattr(args, "bias", True)
         self.gpu = False if args is None else getattr(args, "gpu", False)
         self.att = (args is not None and getattr(args, "method", "base") == "att")
-        if self.att:
-            raise NotImplementedError("method='att' is out of scope (SURVEY 8f)")
-        self.conv_first = GraphConv(input_dim, hidden_dim, add_self, True, 0.0, self.bias)
+        self.conv_first = GraphConv(input_dim, hidden_dim, add_self, True, 0.0, self.bias, att=self.att)
         self.conv_block = nn.ModuleList(
-            [GraphConv(hidden_dim, hidden_dim, add_self, True, dropout, self.bias) for _ in range(num_layers - 2)])
-        self.conv_last = GraphConv(hidden_dim, embedding_dim, add_self, True, 0.0, self.bias)
+            [GraphConv(hidden_dim, hidden_dim, add_self, True, dropout, self.bias, att=self.att) for _ in range(num_layers - 2)])
+        self.conv_last = GraphConv(hidden_dim, embedding_dim, add_self, True, 0.0, self.bias, att=self.att)
         self.act = nn.ReLU()
         self.label_dim = label_dim
         self.pred_input_dim = hidden_dim * (num_layers - 1) + embedding_dim if concat else embedding_dim
@@ -71,6 +75,8 @@ class GcnEncoderGraph(nn.Module):
         for m in self.modules():
             if isinstance(m, GraphConv):
                 init.xavier_uniform_(m.weight.data, gain=nn.init.calculate_gain("relu"))
+                if m.att:
+                    init.xavier_uniform_(m.att_weight.data, gain=nn.init.calculate_gain("relu"))
                 if m.bias is not None:
                     init.constant_(m.bias.data, 0.0)
 
@@ -79,29 +85,29 @@ class GcnEncoderGraph(nn.Module):
         return bn_module(x)
 
     def _layers(self, x, adj):
-        outs = []
-        x, _ = self.conv_first(x, adj)
+        """-> (per-layer outputs, the adjacency each layer aggregated with: adj, or adj scaled by its attention)"""
+        outs, adjs = [], []
+        x, a = self.conv_first(x, adj)
         x = self.act(x)
         if self.bn:
             x = self.apply_bn(x)
-        outs.append(x)
+        outs.append(x); adjs.append(a)
         for conv in self.conv_block:
-            x, _ = conv(x, adj)
+            x, a = conv(x, adj)
             x = self.act(x)
             if self.bn:
                 x = self.apply_bn(x)
-            outs.append(x)
-        x, _ = self.conv_last(x, adj)
-        outs.append(x)
-        return outs
+            outs.append(x); adjs.append(a)
+        x, a = self.conv_last(x, adj)
+        outs.append(x); adjs.append(a)
+        return outs, adjs
 
     def forward(self, x, adj, batch_num_nodes=None, **kwargs):
-        outs = self._layers(x, adj)
+        outs, adjs = self._layers(x, adj)
         pooled = [torch.max(o, dim=1)[0] for o in outs]
         output = torch.cat(pooled, dim=1) if self.concat else pooled[-1]
         self.embedding_tensor = output
-        adj_att = torch.stack([adj] * len(outs), dim=3)
-        return self.pred_model(output), adj_att
+        return self.pred_model(output), torch.stack(adjs, dim=3)   # models.py:296-316
 
     def loss(self, pred, label, type="softmax"):
         return F.cross_entropy(pred, label)
@@ -117,10 +123,9 @@ class GcnEncoderNode(GcnEncoderGraph):
         self.celoss = nn.CrossEntropyLoss()
 
     def forward(self, x, adj, batch_num_nodes=None, **kwargs):
-        outs = self._layers(x, adj)
+        outs, adjs = self._layers(x, adj)
         self.embedding_tensor = torch.cat(outs, dim=2) if self.concat else outs[-1]
-        adj_att = torch.stack([adj] * len(outs), dim=3)
-        return self.pred_model(self.embedding_tensor), adj_att
+        return self.pred_model(self.embedding_tensor), torch.stack(adjs, dim=3)   # models.py:255-267
 
     def loss(self, pred, label):
         return self.celoss(torch.transpose(pred, 1, 2), label)

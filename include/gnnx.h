@@ -50,9 +50,11 @@ typedef struct gx_model_dims {
   int32_t num_layers;  /* num_gc_layers: 2, 3 (reference default) or 4    */
   int32_t flags;       /* GX_MODEL_* bits                               */
 } gx_model_dims;
-#define GX_MODEL_BN 1u /* args.bn (models.py:222-228): per-node standardisation after every hidden ReLU.  num_layers != 3, bn or a
-                        * hidden / output width of 33..128 select the model-variant kernels (node mode and graph mode, mask
+#define GX_MODEL_BN 1u /* args.bn (models.py:222-228): per-node standardisation after every hidden ReLU.  num_layers != 3, bn, att or
+                        * a hidden / output width of 33..128 select the model-variant kernels (node mode and graph mode, mask
                         * optimisation only: no trace / optimiser state / grad) */
+#define GX_MODEL_ATT 2u /* args.method == "att" (models.py:62-68): every layer scales the adjacency by s_ij = P_i . P_j, P = H Wa.
+                         * Set by gx_set_model_att only (gx_set_model refuses it: the attention weights arrive with that call). */
 
 /* Optimisation hyper-parameters: explainer_main.py:143-167 defaults + ExplainModule.coeffs
  * (explainer/explain.py:624-631) + torch.optim.Adam defaults (utils/train_utils.py:10). */
@@ -139,6 +141,13 @@ int gx_sync(gx_handle* h);
  * pred_model.bias (C).  conv_w / conv_b are arrays of num_layers pointers. */
 int gx_set_model(gx_handle* h, const gx_model_dims* dims, const float* const* conv_w,
                  const float* const* conv_b, const float* pred_w, const float* pred_b);
+
+/* Attention model (train.py / explainer_main.py --method att): gx_set_model's arguments plus att_w, num_layers pointers to the
+ * row-major (in, in) conv_first.att_weight / conv_block.i.att_weight / conv_last.att_weight.  GX_MODEL_ATT in dims->flags is
+ * implied.  Runs on the model-variant kernel (mask optimisation only: no trace, optimiser state, GX_INIT_STATE or grad;
+ * no unconstrained mask).  GX_ERR_UNSUPPORTED when the model does not fit the kernel's shared memory. */
+int gx_set_model_att(gx_handle* h, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
+                     const float* const* att_w, const float* pred_w, const float* pred_b);
 
 /* Graph of a node-classification task, replacing Explainer(adj, feat, label, pred) (explain.py:43-62):
  * CSR of the (B=1) adjacency with ascending columns per row (must be symmetric 0/1; self loops are

@@ -1,0 +1,179 @@
+"""gen_att_golden.py -- tests/golden/att_golden.npz by EXECUTING THE UNMODIFIED REFERENCE on attention models (--method att).
+
+The reference's GcnEncoderNode / GcnEncoderGraph built with args.method == "att" (models.py:62-68, reference init: xavier_uniform with
+the ReLU gain on weight and att_weight, models.py:136-150), biases redrawn from N(0, 0.3) so that they matter, explained with
+Explainer.explain (model="exp") in node mode on the rand and syn1 fixture graphs and in graph mode on the 12 graphs of
+graphs_golden.npz.  Needs the reference tree (oracle/ref_harness.py); deterministic:
+    python tools/gen_att_golden.py
+
+Keys (masks at the sub-adjacency entries, row-major, float32; spreads float64):
+  cases                                    the case names
+  <case>_mode / _L / _bn / _hid / _opt / _epochs / _graph        node (0) or graph (1) mode, the model, the optimiser, the fixture graph
+  <case>_w_<W1 .. WL, b1 .., Wa1 .., Wp, bp>                      the model's weights (reference state_dict, renamed)
+  <case>_feat                              node mode: the feature matrix the case used (N, d)
+  <case>_pred, <case>_pred_loop            the model's forward on the fixture graph, and with a self loop on every node (node mode), or
+                                           on each padded graph (graph mode, pred only)
+  <case>_nodes, <case>_n<node>_seed / _nbrs / _mask / _spread   node mode
+  <case>_g<g>_mask / _spread               graph mode (M0 seeds: graphs_golden.npz g<g>_seed)
+The spread of a case is the reproducibility of the reference itself: the largest distance from the reference's mask of the
+line-by-line port (tests/att_oracle.py) run with every M0 entry nudged by +-1 ulp (NUDGES draws), and of the same port in fp64.
+The port must reproduce every reference mask to within max(1e-6, 3 x spread): below 1e-6 wherever the trajectory does not amplify
+rounding (every node case); a few graph trajectories do (graph 5 of graphs_bn_L4, graphs 0 and 10 at 100 epochs), and there the port
+lands within the reference's own spread.
+"""
+import os
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "oracle"))
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import att_oracle as AO  # noqa: E402
+import gnnx_oracle as O  # noqa: E402
+import ref_harness  # noqa: E402
+from gen_golden import OUT, train_args  # noqa: E402
+
+NUDGES = 3
+# name: (graph, nodes, L, bn, hid, d (None: the fixture's features), opt, epochs)
+NODE_CASES = {
+    "rand_L3_e30": ("rand", [0, 7, 33, 100], 3, False, 20, None, "adam", 30),
+    "rand_L3_e100": ("rand", [0, 7, 33, 100], 3, False, 20, None, "adam", 100),
+    "rand_bn_L2": ("rand", [0, 7, 33, 100], 2, True, 20, None, "adam", 30),
+    "rand_L4": ("rand", [0, 33, 149], 4, False, 20, None, "adam", 30),
+    "rand_w64": ("rand", [0, 7, 100], 3, False, 64, None, "adam", 30),
+    "rand_d128": ("rand", [0, 7, 100], 3, False, 20, 128, "adam", 30),
+    "rand_sgd": ("rand", [0, 7, 33], 3, False, 20, None, "sgd", 30),
+    "syn1_L3": ("syn1", [3, 13, 300, 550], 3, False, 20, None, "adam", 30),
+}
+# name: (L, bn, epochs)
+GRAPH_CASES = {"graphs_L3_e30": (3, False, 30), "graphs_L3_e100": (3, False, 100), "graphs_bn_L4": (4, True, 30)}
+
+
+def _nudged(M0, s, salt):
+    rng = np.random.default_rng(1000 * s + salt)
+    up = rng.integers(0, 2, M0.shape).astype(bool)
+    return np.where(up, np.nextafter(M0, np.float32(np.inf)), np.nextafter(M0, np.float32(-np.inf))).astype(np.float32)
+
+
+def _spread(port, M0, ref, ei, ej, salt, what):
+    spread = O.rel_l2(port(M0, torch.float64)[ei, ej], ref)
+    for s in range(NUDGES):
+        spread = max(spread, O.rel_l2(port(_nudged(M0, s, salt), torch.float)[ei, ej], ref))
+    err = O.rel_l2(port(M0, torch.float)[ei, ej], ref)
+    assert err <= max(1e-6, 3 * spread), (what, err, spread)
+    return spread
+
+
+def _att_model(R, cls, d, hid, C, L, bn, seed):
+    torch.manual_seed(seed)
+    model = cls(d, hid, hid, C, L, bn=bn, args=train_args(input_dim=d, hidden_dim=hid, output_dim=hid, num_gc_layers=L, bn=bn,
+                                                           method="att"))
+    with torch.no_grad():
+        for name, p_ in model.named_parameters():
+            if name.endswith("bias"):
+                p_.normal_(0.0, 0.3)
+    model.eval()
+    sd = model.state_dict()
+    keys = ["conv_first"] + ["conv_block.%d" % i for i in range(L - 2)] + ["conv_last"]
+    W = {}
+    for l, k in enumerate(keys, 1):
+        W["W%d" % l] = sd[k + ".weight"].numpy().astype(np.float32)
+        W["b%d" % l] = sd[k + ".bias"].numpy().astype(np.float32)
+        W["Wa%d" % l] = sd[k + ".att_weight"].numpy().astype(np.float32)
+    W["Wp"] = sd["pred_model.weight"].numpy().astype(np.float32)
+    W["bp"] = sd["pred_model.bias"].numpy().astype(np.float32)
+    return model, W
+
+
+def gen_node_case(R, out, name, graph, nodes, L, bn, hid, d_feat, opt, epochs, seed):
+    g = np.load(os.path.join(OUT, graph + "_graph.npz"))
+    gold = np.load(os.path.join(OUT, graph + "_golden.npz"))
+    N, C = int(g["N"]), g["Wp"].shape[0]
+    feat = g["feat"].astype(np.float32) if d_feat is None else np.random.default_rng(seed).normal(size=(N, d_feat)).astype(np.float32)
+    d = feat.shape[1]
+    adj = np.zeros((1, N, N)); e = g["edges"]; adj[0, e[:, 0], e[:, 1]] = 1; adj[0, e[:, 1], e[:, 0]] = 1
+    model, W = _att_model(R, R.models.GcnEncoderNode, d, hid, C, L, bn, seed)
+    with torch.no_grad():
+        pred, _ = model(torch.tensor(feat[None]), torch.tensor(adj, dtype=torch.float))
+        pred_loop, _ = model(torch.tensor(feat[None]), torch.tensor(adj + np.eye(N)[None], dtype=torch.float))
+    eargs = ref_harness.explainer_args(dataset=graph, num_epochs=epochs, num_gc_layers=L, bn=bn, opt=opt, method="att", hidden_dim=hid,
+                                       output_dim=hid)
+    with ref_harness.quiet():
+        ex = R.explain.Explainer(model=model, adj=adj, feat=feat[None].astype(np.float64), label=g["label"][None], pred=pred.numpy(),
+                                 train_idx=list(range(N)), args=eargs, writer=None, print_training=False, graph_idx=-1)
+    out.update({"%s_w_%s" % (name, k): v for k, v in W.items()})
+    out.update({name + "_mode": np.int64(0), name + "_L": np.int64(L), name + "_bn": np.int64(bn), name + "_hid": np.int64(hid),
+                name + "_opt": np.str_(opt), name + "_epochs": np.int64(epochs), name + "_graph": np.str_(graph),
+                name + "_feat": feat, name + "_pred": pred[0].numpy(), name + "_pred_loop": pred_loop[0].numpy(),
+                name + "_nodes": np.asarray(nodes, np.int64)})
+    hp = O.default_hparams(num_epochs=epochs, opt=opt)
+    for node in nodes:
+        seed_n = int(gold["n%d_seed" % node]) if ("n%d_seed" % node) in gold.files else 7000 + node
+        with ref_harness.quiet():
+            idx, sub_adj, sub_feat, sub_label, nbrs = ex.extract_neighborhood(node, 0)
+        M0 = O.draw_m0(len(nbrs), seed=seed_n)
+        torch.manual_seed(seed_n)
+        with ref_harness.quiet():
+            masked = np.asarray(ex.explain(node, graph_idx=0))
+        ei, ej = np.nonzero(sub_adj)
+        ref = masked[ei, ej]
+        pl = np.argmax(pred[0].numpy()[nbrs], axis=1)
+        gt = int(np.asarray(sub_label)[idx])
+        A = np.asarray(sub_adj, np.float64)
+        port = lambda M, dt: AO.explain_att_torch(A, np.asarray(sub_feat, np.float32), gt, pl, idx, W, M, hp, bn=bn, dtype=dt)
+        key = "%s_n%d" % (name, node)
+        out[key + "_seed"] = np.int64(seed_n)
+        out[key + "_nbrs"] = np.asarray(nbrs, np.int32)
+        out[key + "_mask"] = ref.astype(np.float32)
+        out[key + "_spread"] = np.float64(_spread(port, M0, ref, ei, ej, node, key))
+    print("  %s: spreads %s" % (name, ["%.1e" % out["%s_n%d_spread" % (name, v)] for v in nodes]), flush=True)
+
+
+def gen_graph_case(R, out, name, L, bn, epochs, seed):
+    gg = np.load(os.path.join(OUT, "graphs_golden.npz"))
+    G_n, n = int(gg["num_graphs"]), int(gg["max_nodes"])
+    adj, feat, label = gg["adj"].astype(np.float64), gg["feat"].astype(np.float32), gg["label"].astype(np.int64)
+    d, C = feat.shape[2], gg["Wp"].shape[0]
+    model, W = _att_model(R, R.models.GcnEncoderGraph, d, 20, C, L, bn, seed)
+    with torch.no_grad():
+        pred = np.stack([model(torch.tensor(feat[g:g + 1]), torch.tensor(adj[g:g + 1], dtype=torch.float))[0][0].numpy()
+                         for g in range(G_n)])
+    eargs = ref_harness.explainer_args(dataset="graphs", num_epochs=epochs, num_gc_layers=L, bn=bn, method="att")
+    with ref_harness.quiet():
+        ex = R.explain.Explainer(model=model, adj=torch.tensor(adj, dtype=torch.float), feat=torch.tensor(feat),
+                                 label=torch.tensor(label), pred=pred[None], train_idx=list(range(G_n)), args=eargs,
+                                 writer=None, print_training=False, graph_mode=True, graph_idx=0)
+    out.update({"%s_w_%s" % (name, k): v for k, v in W.items()})
+    out.update({name + "_mode": np.int64(1), name + "_L": np.int64(L), name + "_bn": np.int64(bn), name + "_hid": np.int64(20),
+                name + "_opt": np.str_("adam"), name + "_epochs": np.int64(epochs), name + "_graph": np.str_("graphs"),
+                name + "_pred": pred})
+    hp = O.default_hparams(num_epochs=epochs)
+    for g in range(G_n):
+        seed_g = int(gg["g%d_seed" % g])
+        M0 = O.draw_m0(n, seed=seed_g)
+        torch.manual_seed(seed_g)
+        with ref_harness.quiet():
+            masked = np.asarray(ex.explain(node_idx=0, graph_idx=g, graph_mode=True))
+        ei, ej = np.nonzero(adj[g])
+        ref = masked[ei, ej]
+        port = lambda M, dt: AO.explain_att_torch(adj[g], feat[g], int(label[g]), None, 0, W, M, hp, graph_mode=True, bn=bn, dtype=dt)
+        out["%s_g%d_mask" % (name, g)] = ref.astype(np.float32)
+        out["%s_g%d_spread" % (name, g)] = np.float64(_spread(port, M0, ref, ei, ej, 100 + g, "%s_g%d" % (name, g)))
+    print("  %s: spreads %s" % (name, ["%.1e" % out["%s_g%d_spread" % (name, g)] for g in range(G_n)]), flush=True)
+
+
+def gen(R):
+    out = {"cases": np.asarray(list(NODE_CASES) + list(GRAPH_CASES))}
+    for k, (name, c) in enumerate(NODE_CASES.items()):
+        gen_node_case(R, out, name, *c, seed=600 + k)
+    for k, (name, c) in enumerate(GRAPH_CASES.items()):
+        gen_graph_case(R, out, name, *c, seed=700 + k)
+    np.savez_compressed(os.path.join(OUT, "att_golden.npz"), **out)
+    print("  att golden written")
+
+
+if __name__ == "__main__":
+    torch.set_num_threads(8)
+    gen(ref_harness.load())

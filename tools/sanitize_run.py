@@ -2,7 +2,7 @@
 """Small invocation of every kernel for compute-sanitizer (racecheck / memcheck / synccheck are ~100x slower than a plain run):
     compute-sanitizer --tool racecheck python tools/sanitize_run.py
 k-hop extraction + shared-memory kernel on a mix of task sizes (syn1: hub node 0 and tiny tasks), the streaming kernel (forced),
-the gradient baseline, graph mode, densify, neighbourhood rows, the unconstrained (dense) kernel.  A few epochs each."""
+the gradient baseline, graph mode, densify, neighbourhood rows, the unconstrained (dense) kernel, attention models.  A few epochs each."""
 import os
 import sys
 
@@ -19,7 +19,7 @@ EPOCHS = int(os.environ.get("SAN_EPOCHS", "4"))
 
 
 def main():
-    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster", "dense"]
+    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster", "dense", "att"]
     fx = util.load_fixture("syn1")
     if "node" in which:
         eng = util.make_engine(fx)
@@ -139,6 +139,38 @@ def main():
         out = np.zeros(int(eoff[-1]), np.float32)
         eng.explain_graphs_unconstrained(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=5), None, out)
         print("dense ok graph", float(out.sum()))
+        eng.close()
+    if "att" in which:   # explain_var.cu's attention path: node mode (hub and small tasks; with hid = 128 the attention weights are read
+        # through L2 while the conv weights stay in shared memory), graph mode, the model forward
+        rng = np.random.default_rng(7)
+        sc = lambda *s_: (rng.normal(size=s_) * 0.3).astype(np.float32)
+        d0, C0 = fx.feat.shape[1], fx.weights["Wp"].shape[0]
+        for hid, L, bn in ((20, 3, False), (128, 3, True)):
+            dims = [d0] + [hid] * L
+            w = {}
+            for l in range(1, L + 1):
+                w["W%d" % l] = sc(dims[l - 1], dims[l]); w["b%d" % l] = sc(dims[l]); w["Wa%d" % l] = sc(dims[l - 1], dims[l - 1])
+            w["Wp"] = sc(C0, hid * L); w["bp"] = sc(C0)
+            att = [w["Wa%d" % l] for l in range(1, L + 1)]
+            eng = gnnx.Engine(0)
+            eng.set_model(w, num_layers=L, bn=bn, att=att)
+            eng.set_graph_csr(fx.rowptr, fx.col, fx.feat, fx.label, fx.pred_label)
+            plan = eng.plan_nodes([0, 300, 5, 683], L)
+            out = np.zeros(plan.total_edges, np.float32)
+            eng.explain_nodes_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=8), None, out)
+            pred = eng.model_forward() if hid <= 32 else np.zeros(1)
+            print("att ok node", hid, L, bn, float(out.sum()), float(pred.sum()))
+            eng.close()
+        g = np.load(util.GOLDEN + "/graphs_golden.npz")
+        dg, Cg = g["feat"].shape[2], g["Wp"].shape[0]
+        w = dict(W1=sc(dg, 20), b1=sc(20), W2=sc(20, 20), b2=sc(20), W3=sc(20, 20), b3=sc(20), Wp=sc(Cg, 60), bp=sc(Cg))
+        eng = gnnx.Engine(0)
+        eng.set_model(w, num_layers=3, att=[sc(dg, dg), sc(20, 20), sc(20, 20)])
+        eng.set_graph_batch(g["adj"], g["feat"], g["label"])
+        eoff = eng.plan_graphs([0, 3, 5])
+        out = np.zeros(int(eoff[-1]), np.float32)
+        eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=9), None, out)
+        print("att ok graph", float(out.sum()))
         eng.close()
     if "misc" in which:
         eng = util.make_engine(fx)
