@@ -224,7 +224,7 @@ int launch_var_batch(gx_handle* h, const char* who, int graph_mode, const GxHpar
   return GX_OK;
 }
 
-// Model variant (num_gc_layers 2 / 4, --bn, widths 33..128, attention): explain_var.cu, true widths (a zero-padded column would enter
+// Model variant (num_gc_layers 2 / 4, --bn, widths 33..128, attention, inputs wider than 128): explain_var.cu, true widths (a zero-padded column would enter
 // the bn statistics).  att_w != nullptr: an attention model, each layer's (in, in) attention weights right after its conv weights
 // (gx_att_weight).  The widths were checked by the caller.
 static int set_variant_model(gx_handle* h, const char* who, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
@@ -276,8 +276,8 @@ static int check_model_dims(const char* who, const gx_model_dims* dims) {
     gx_set_error("%s: hidden_dim=%d output_dim=%d; this build supports widths up to 128 (tuned kernels up to 32, the variant kernel beyond)", who, dims->hidden_dim, dims->embed_dim);
     return GX_ERR_UNSUPPORTED;
   }
-  if (dims->input_dim < 1 || dims->input_dim > 128) {
-    gx_set_error("%s: input_dim=%d outside [1,128] supported by the shared-memory kernel", who, dims->input_dim);
+  if (dims->input_dim < 1 || dims->input_dim > GX_VAR_WIDE_MAX) {
+    gx_set_error("%s: input_dim=%d outside [1,%d] (inputs wider than 128 run the variant kernel's wide path)", who, dims->input_dim, GX_VAR_WIDE_MAX);
     return GX_ERR_UNSUPPORTED;
   }
   if (dims->num_classes < 1) { gx_set_error("%s: num_classes < 1", who); return GX_ERR_INVALID; }
@@ -449,7 +449,7 @@ int gx_set_model(gx_handle* h, const gx_model_dims* dims, const float* const* co
   if (rc != GX_OK) return rc;
   if (dims->flags & GX_MODEL_ATT) { gx_set_error("gx_set_model: GX_MODEL_ATT models are set with gx_set_model_att (it takes the attention weights)"); return GX_ERR_INVALID; }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
-  if (dims->num_layers != 3 || (dims->flags & GX_MODEL_BN) || dims->hidden_dim > 32 || dims->embed_dim > 32)
+  if (dims->num_layers != 3 || (dims->flags & GX_MODEL_BN) || dims->hidden_dim > 32 || dims->embed_dim > 32 || dims->input_dim >= GX_VAR_WIDE_MIN)
     return set_variant_model(h, "gx_set_model", dims, conv_w, conv_b, nullptr, pred_w, pred_b);
   // The kernels are instantiated for the reference default 20/20 and for 32/32; any other width <= 32 is
   // zero-padded to 32.  Padding is exact: a padded output column is 0*W + 0 = 0, contributes nothing to the
@@ -501,6 +501,10 @@ int gx_set_model_att(gx_handle* h, const gx_model_dims* dims, const float* const
   if (!h || !dims || !conv_w || !att_w || !pred_w || !pred_b) { gx_set_error("gx_set_model_att: NULL argument"); return GX_ERR_INVALID; }
   const int rc = check_model_dims("gx_set_model_att", dims);
   if (rc != GX_OK) return rc;
+  if (dims->input_dim >= GX_VAR_WIDE_MIN) {
+    gx_set_error("gx_set_model_att: input_dim=%d; attention models are built for inputs up to 128 wide (layer 1's attention matrix is input_dim x input_dim)", dims->input_dim);
+    return GX_ERR_UNSUPPORTED;
+  }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
   return set_variant_model(h, "gx_set_model_att", dims, conv_w, conv_b, att_w, pred_w, pred_b);
 }

@@ -24,7 +24,16 @@
 // phase before the gather (Fl = Pl | Sl | gather with a s); the backward adds, after the row phase, t_ij = dL/dZ_i . H_{l-1}[j] per
 // slot, the pair weights a_ij (t_ij + t_ji), and dL/dP = sum_j a_ij (t_ij + t_ji) P_j, whose dL/dP Wa^T joins dL/dH_{l-1} (layer 1:
 // dL/dsF).  The edge phase then uses dL/da_ij + dL/da_ji = sum_l s_ij (t_ij + t_ji) from the stored s and t.
+// Wide inputs (kWide, 128 < d <= 4096) contract layer 1 in the other order, A_m (X (sF (.) W1)) (DESIGN section 13), so that every per-edge
+// step is hid-wide and the d-wide work is two products per epoch on the tensor cores:
+//   F0  P = X B with B = sF (.) W1 formed on the fly (3xTF32 mma.sync), every row of the task;
+//   F1  y_i = b1 + sum_j a_ij P_j, then the usual row epilogue;
+//   B1  dY1 of layer 1's rows, then dP_j = sum_i a_ij dY1_i over every row j (the leading columns of j that are layer-1 rows);
+//   B0  G = X^T dP (3xTF32), dL/dsF_f = sum_c W1_fc G_fc;
+//   P   layer 1's pair term <dY1_i, P_j> + <dY1_j, P_i> replaces the d-wide dots.
+// The feature-mask state and the products live in the task slab and W1 is read through L2, so shared memory does not grow with d.
 #include "explain_var_common.cuh"
+#include "mma_tf32.cuh"
 
 namespace {
 
@@ -156,9 +165,39 @@ __device__ __forceinline__ void att_backward_edges(int win, int ldp, int nrow, i
   __syncthreads();
 }
 
+// ---------------------------------------------------------------------------------------------------------------------- wide inputs
+// C = A B (M x N, row stride ldc) on the tensor cores, 3xTF32 (mma_tf32.cuh): one 16 x 8 tile per warp at a time, the k steps of a tile
+// in ascending order, so the product is deterministic.  a(r, k) and b(k, c) return the operands and 0 outside the matrices.
+template <typename FA, typename FB>
+__device__ __forceinline__ void wide_mma(int M, int N, int K, FA a, FB b, float* C, int ldc, int warp, int nwarps, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  const int tn = (N + 7) / 8, tiles = (M + 15) / 16 * tn;
+  for (int tile = warp; tile < tiles; tile += nwarps) {
+    const int m0 = tile / tn * 16, n0 = tile % tn * 8;
+    float c[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int k0 = 0; k0 < K; k0 += 8) {
+      uint32_t ah[4], al[4], bh0, bl0, bh1, bl1;
+      tf32_split(a(m0 + g, k0 + t), ah[0], al[0]);
+      tf32_split(a(m0 + g + 8, k0 + t), ah[1], al[1]);
+      tf32_split(a(m0 + g, k0 + t + 4), ah[2], al[2]);
+      tf32_split(a(m0 + g + 8, k0 + t + 4), ah[3], al[3]);
+      tf32_split(b(k0 + t, n0 + g), bh0, bl0);
+      tf32_split(b(k0 + t + 4, n0 + g), bh1, bl1);
+      mma_tf32(c, al, bh0, bh1);   // the small terms first
+      mma_tf32(c, ah, bl0, bl1);
+      mma_tf32(c, ah, bh0, bh1);
+    }
+    const int r = m0 + g, col = n0 + 2 * t;
+    if (r < M && col < N) C[(int64_t)r * ldc + col] = c[0];
+    if (r < M && col + 1 < N) C[(int64_t)r * ldc + col + 1] = c[1];
+    if (r + 8 < M && col < N) C[(int64_t)(r + 8) * ldc + col] = c[2];
+    if (r + 8 < M && col + 1 < N) C[(int64_t)(r + 8) * ldc + col + 1] = c[3];
+  }
+}
+
 // The minimum-blocks bound 0 is the compiler's default: node mode is capped at 128 registers (some instantiations spill); graph mode
 // lets the small default-width model fit two CTAs per SM.
-template <bool kGraph, bool kBn, int KW, bool kAtt>
+template <bool kGraph, bool kBn, int KW, bool kAtt, bool kWide>
 __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1) : 0) explain_var_kernel(const VarArgs A) {
   extern __shared__ __align__(16) float sm[];
   __shared__ int s_task;
@@ -171,7 +210,7 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
   const int dp = gx_round_up(d, 4);
   const int PD = hid * (L - 1) + embw;
   const bool ieee = (hp.flags & GX_HP_IEEE_EDGE) != 0;
-  const VarSmem S = var_smem(d, L, hid, embw, C, nwarps, kAtt ? 1 : 0);
+  const VarSmem S = var_smem_of<kWide>(d, L, hid, embw, C, nwarps, kAtt ? 1 : 0);
   float* const sF = sm + S.sF; float* const Fm = sm + S.F; float* const mF = sm + S.mF; float* const vF = sm + S.vF;
   float* const zs = sm + S.zs + warp * S.zlen;
   float* const gFp = sm + S.gFp;
@@ -185,7 +224,7 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
   auto wout_of = [&](int l) { return l == L - 1 ? embw : hid; };
 
   const float* Wl[GX_MAX_LAYERS];   // conv weights: shared memory when they fit, else global (L2 resident)
-  var_stage_model(m, S, sm, Wl, tid, NT);
+  var_stage_model<kWide>(m, S, sm, Wl, tid, NT);
   const float* Wal[kAtt ? GX_MAX_LAYERS : 1];  // attention weights (kAtt), staged like Wl
   if constexpr (kAtt) var_stage_att(m, S, sm, Wal, tid, NT);
   if constexpr (kGraph) {
@@ -221,7 +260,7 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
     }
     auto rows = [&](int l) { if constexpr (kGraph) return n; else return R[l]; };
     auto rin = [&](int l) { if constexpr (kGraph) return n; else return R[l - 1]; };   // input rows of layer l
-    const GxVarLayout Lo = gx_make_var_layout(n, n2, e1, kGraph ? 0 : np, d, L, VW, kAtt ? 1 : 0, Tp->e_d);
+    const GxVarLayout Lo = gx_make_var_layout(n, n2, e1, kGraph ? 0 : np, d, L, VW, kAtt ? 1 : 0, Tp->e_d, kWide ? 1 : 0);
     // layer 1's input rows: the graph's features (node mode), this graph's padded rows (graph mode); both indexed by lo2gid
     const float* const feat = kGraph ? A.gb.feat + (int64_t)Tp->node * A.gb.max_nodes * d : A.g.feat;
     const int32_t* __restrict__ lo2gid = A.plan.lo2gid + node_off;
@@ -243,12 +282,20 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
     auto tl = [&](int l) { return slab + Lo.t + (int64_t)(l - 1) * e1; };
     float* const cw = slab + Lo.cw; float* const dHa = slab + Lo.dHa;
     float2* const mm = MM + np; float2* const vv = mm + np; float2* const SS = vv + np;
+    // the feature-mask state: shared memory, or the slab for wide inputs (kWide), which also holds P = X B, dY1, dP = A_m^T dY1,
+    // G = X^T dP and dL/dsF
+    float* const fsF = kWide ? slab + Lo.fm : sF; float* const fF = kWide ? slab + Lo.fm + dp : Fm;
+    float* const fmF = kWide ? slab + Lo.fm + 2 * dp : mF; float* const fvF = kWide ? slab + Lo.fm + 3 * dp : vF;
+    float* const gFw = slab + Lo.fm + 4 * dp;
+    float* const XB = slab + Lo.XB; float* const dY1 = slab + Lo.dY1; float* const dP = slab + Lo.dP; float* const Gw = slab + Lo.G;
+    const float* const W1 = m.W[0];
+    auto xat = [=](int r, int f) { return r < n && f < d ? __ldg(feat + (int64_t)lo2gid[r] * d + f) : 0.f; };   // X of the task, level order
     const float nn = (float)Tp->n_norm * (float)Tp->n_norm;
     const float ent_over_nn = hp.c_ent / nn;
     const float lap_over_nn = hp.c_lap / nn;
 
     for (int f = tid; f < dp; f += NT) {
-      sF[f] = 0.5f; Fm[f] = 0.f; mF[f] = 0.f; vF[f] = 0.f;   // feat_mask = 0 (explain.py:633-643)
+      fsF[f] = 0.5f; fF[f] = 0.f; fmF[f] = 0.f; fvF[f] = 0.f;   // feat_mask = 0 (explain.py:633-643)
       if (hp.out_iter == 0 && f < d && A.out_feat != nullptr) A.out_feat[(int64_t)task_id * d + f] = 0.5f;
     }
     {
@@ -264,8 +311,8 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
         SS[p] = make_float2(Si, Sj);
         const float a0 = 0.5f * (Si + Sj);  // explain.py:665-678
         const int i = pi[p], j = pj[p];
-        if (kGraph || i < n2) a[ppij[p]] = a0;
-        if (kGraph || j < n2) a[ppji[p]] = a0;
+        if (kGraph || kWide || i < n2) a[ppij[p]] = a0;
+        if (kGraph || kWide || j < n2) a[ppji[p]] = a0;
         if constexpr (!kGraph) {   // no Laplacian term in graph mode (explain.py:787-788)
           const float yd = (float)__ldg(A.g.pred_label + lo2gid[i]) - (float)__ldg(A.g.pred_label + lo2gid[j]);
           lapg[p] = lap_over_nn * yd * yd;   // d/dA_ij + d/dA_ji of y^T (D - A) y / n^2 (explain.py:780-793)
@@ -277,6 +324,11 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
 
     for (int it = 1; it <= hp.iters; ++it) {
       // ---------------------------------------------------------------- forward, layer by layer        (models.py:58-80,230-267)
+      if constexpr (kWide) {   // F0: P = X (sF (.) W1) on every row of the task
+        wide_mma(n, hid, d, xat, [&](int f, int c) { return f < d && c < hid ? fsF[f] * __ldg(W1 + (int64_t)f * hid + c) : 0.f; }, XB, VW,
+                 warp, nwarps, lane);
+        __syncthreads();
+      }
       for (int l = 1; l <= L; ++l) {
         const int win = win_of(l - 1), wout = wout_of(l - 1);
         const float* const Ws = Wl[l - 1]; const float* const bsm = sm + S.b[l - 1];
@@ -288,6 +340,22 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
         }
         for (int i = warp; i < rows(l); i += nwarps) {
           const int r0 = irp[i], r1 = irp[i + 1];
+          if constexpr (kWide) {
+            if (l == 1) {   // F1: y = b1 + sum_j a_ij P_j
+              float y[KW];
+#pragma unroll
+              for (int k = 0; k < KW; ++k) y[k] = lane + 32 * k < wout ? bsm[lane + 32 * k] : 0.f;
+              for (int e = r0; e < r1; ++e) {
+                const float ae = a[e];
+                const float* const Pj = XB + (int64_t)icol[e] * VW;
+#pragma unroll
+                for (int k = 0; k < KW; ++k)
+                  if (lane + 32 * k < wout) y[k] = fmaf(ae, Pj[lane + 32 * k], y[k]);
+              }
+              var_row_epilogue<kBn, KW>(y, wout, l, L, i, Yh, Hh, VW, qn, istd, lane);
+              continue;
+            }
+          }
           if (l == 1) var_gather_feat(r0, r1, icol, ag, feat, lo2gid, d, sF, U + (int64_t)i * dp, zs, lane);
           else var_gather_hidden<KW>(r0, r1, icol, ag, Hh(l - 1), win, zs, lane);
           var_row_forward<kBn, KW>(zs, win, Ws, wout, bsm, l, L, i, Yh, Hh, VW, qn, istd, lane);
@@ -307,7 +375,8 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
         }
         var_readout_tail(emb, Wpp, bpp, C, PD, gt, logit, dEmb, lane);
       }
-      for (int idx = tid; idx < nwarps * dp; idx += NT) gFp[idx] = 0.f;
+      if constexpr (!kWide)
+        for (int idx = tid; idx < nwarps * dp; idx += NT) gFp[idx] = 0.f;
       __syncthreads();
       // ---------------------------------------------------------------- backward, layer by layer
       for (int l = L; l >= 1; --l) {
@@ -332,12 +401,45 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
             yh[k] = Yh(l)[(int64_t)i * VW + c];
           }
           var_row_backward<kBn, KW>(g, yh, l, L, i, Hh, VW, qn, istd, wout, zs, lane);
+          if constexpr (kWide) {
+            if (l == 1) {   // B1: keep dY1
+#pragma unroll
+              for (int k = 0; k < KW; ++k) dY1[(int64_t)i * VW + lane + 32 * k] = lane + 32 * k < wout ? zs[lane + 32 * k] : 0.f;
+              __syncwarp();
+              continue;
+            }
+          }
           // dZ[f] = sum_c dY[c] W[f][c]
           if (l == 1) var_first_layer_dz(zs, Ws, d, wout, U + (int64_t)i * dp, sF, gFp + warp * dp, dZ1 + (int64_t)i * dp, lane);
           else var_hidden_dz<KW>(zs, Ws, win, wout, dZ(l) + (int64_t)i * VW, lane);
           __syncwarp();
         }
         __syncthreads();
+        if constexpr (kWide) {
+          if (l == 1) {
+            // B1: dP_j = sum_i a_ij dY1_i over j's leading columns that are layer-1 rows (A_m symmetric), every row j of the task
+            for (int j = warp; j < n; j += nwarps) {
+              float g[KW];
+#pragma unroll
+              for (int k = 0; k < KW; ++k) g[k] = 0.f;
+              var_gather_back<KW>(irp[j], irp[j + 1], icol, a, dY1, wout, rows(1), g, lane);
+#pragma unroll
+              for (int k = 0; k < KW; ++k) dP[(int64_t)j * VW + lane + 32 * k] = g[k];
+            }
+            __syncthreads();
+            // B0: G = X^T dP, then dL/dsF_f = sum_c W1_fc G_fc
+            wide_mma(d, hid, n, [&](int f, int r) { return xat(r, f); }, [&](int r, int c) { return r < n && c < hid ? dP[(int64_t)r * VW + c] : 0.f; },
+                     Gw, VW, warp, nwarps, lane);
+            __syncthreads();
+            for (int f = warp; f < d; f += nwarps) {
+              float t = 0.f;
+              for (int c = lane; c < hid; c += 32) t = fmaf(__ldg(W1 + (int64_t)f * hid + c), Gw[(int64_t)f * VW + c], t);
+              t = warp_sum(t);
+              if (lane == 0) gFw[f] = t;
+            }
+            __syncthreads();
+          }
+        }
         if constexpr (kAtt)
           att_backward_edges(win, l == 1 ? dp : VW, rows(l), rin(l), kGraph ? n : n2, np, d, feat, lo2gid, l == 1 ? dZ1 : dZ(l),
                              l == 1 ? nullptr : Hh(l - 1), VW, Wal[l - 1], irp, icol, a, pi, pj, ppij, ppji, Pl(l), tl(l), cw, dHa,
@@ -350,14 +452,16 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
         const bool last = (it == hp.out_iter);   // the mask built after this update is the one the reference returns
         for (int f = tid; f < d; f += NT) {
           float gsum = 0.f;
-          for (int w = 0; w < nwarps; ++w) gsum += gFp[w * dp + f];
-          const float s = sF[f];
+          if constexpr (kWide) gsum = gFw[f];
+          else
+            for (int w = 0; w < nwarps; ++w) gsum += gFp[w * dp + f];
+          const float s = fsF[f];
           const float g = s * (1.f - s) * (gsum + hp.c_feat_size / (float)d);
-          float mf = mF[f], vf = vF[f], Fv = Fm[f];
+          float mf = fmF[f], vf = fvF[f], Fv = fF[f];
           var_feat_update(hp, g, Fv, mf, vf, step, bc2s);
-          mF[f] = mf; vF[f] = vf; Fm[f] = Fv;
+          fmF[f] = mf; fvF[f] = vf; fF[f] = Fv;
           const float sn = sigmoid_f(Fv);
-          sF[f] = sn;   // (the edge dots below use dZ1 (.) sF stored in the backward, not this value)
+          fsF[f] = sn;   // (the edge dots below use dZ1 (.) sF stored in the backward, not this value)
           if (last && A.out_feat != nullptr) A.out_feat[(int64_t)task_id * d + f] = sn;
         }
         for (int p = tid; p < np; p += NT) {
@@ -372,7 +476,7 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
               const float tij = ri ? tl(l)[ppij[p]] : 0.f, tji = rj ? tl(l)[ppji[p]] : 0.f;
               Gd = fmaf(sl(l)[ppij[p]], tij + tji, Gd);
             }
-          } else if constexpr (kGraph) {   // no Laplacian term; every row at every layer, both directions of a layer in one sum
+          } else if constexpr (kGraph && !kWide) {   // no Laplacian term; every row at every layer, both directions of a layer in one sum
             Gd = 0.f;
             {
               const float* xi = feat + (int64_t)lo2gid[i] * d; const float* xj = feat + (int64_t)lo2gid[j] * d;
@@ -388,7 +492,7 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
               for (int f = 0; f < hid; ++f) t = fmaf(dZl[(int64_t)j * VW + f], Hp[(int64_t)i * VW + f], t);
               Gd += t;
             }
-          } else {   // only the rows of layer l, the two directions added one by one
+          } else if constexpr (!kWide) {   // only the rows of layer l, the two directions added one by one
             Gd = lapg[p];
             if (i < R[1]) {
               float t = 0.f;
@@ -407,6 +511,24 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
               if (i < R[l]) { float t = 0.f; for (int f = 0; f < hid; ++f) t = fmaf(dZl[(int64_t)i * VW + f], Hp[(int64_t)j * VW + f], t); Gd += t; }
               if (j < R[l]) { float t = 0.f; for (int f = 0; f < hid; ++f) t = fmaf(dZl[(int64_t)j * VW + f], Hp[(int64_t)i * VW + f], t); Gd += t; }
             }
+          } else {   // wide inputs: as the two branches above, with layer 1's term <dY1_i, P_j> + <dY1_j, P_i> (hid-wide)
+            auto dot = [&](const float* u, const float* v, int w) { float t = 0.f; for (int c = 0; c < w; ++c) t = fmaf(u[c], v[c], t); return t; };
+            const float* const Yi = dY1 + (int64_t)i * VW; const float* const Yj = dY1 + (int64_t)j * VW;
+            const float* const Pi = XB + (int64_t)i * VW; const float* const Pj = XB + (int64_t)j * VW;
+            if constexpr (kGraph) {
+              Gd = dot(Yi, Pj, hid) + dot(Yj, Pi, hid);
+              for (int l = 2; l <= L; ++l) {
+                const float* const dZl = dZ(l); const float* const Hp = Hh(l - 1);
+                Gd += dot(dZl + (int64_t)i * VW, Hp + (int64_t)j * VW, hid) + dot(dZl + (int64_t)j * VW, Hp + (int64_t)i * VW, hid);
+              }
+            } else {
+              Gd = lapg[p];
+              for (int l = 1; l <= L; ++l) {
+                const float* const dZl = l == 1 ? dY1 : dZ(l); const float* const Hp = l == 1 ? XB : Hh(l - 1);
+                if (i < R[l]) Gd += dot(dZl + (int64_t)i * VW, Hp + (int64_t)j * VW, hid);
+                if (j < R[l]) Gd += dot(dZl + (int64_t)j * VW, Hp + (int64_t)i * VW, hid);
+              }
+            }
           }
           Gd *= 0.5f;  // sym_mask = (S + S^T)/2 (explain.py:671)
           float2 Mv = MM[p];
@@ -419,8 +541,8 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
           const float2 Sn = make_float2(sigmoid_fast(Mv.x, ieee), sigmoid_fast(Mv.y, ieee));
           MM[p] = Mv; mm[p] = m2; vv[p] = v2; SS[p] = Sn;
           const float an = 0.5f * (Sn.x + Sn.y);
-          if (kGraph || i < n2) a[ppij[p]] = an;
-          if (kGraph || j < n2) a[ppji[p]] = an;
+          if (kGraph || kWide || i < n2) a[ppij[p]] = an;
+          if (kGraph || kWide || j < n2) a[ppji[p]] = an;
           if (last) { A.out_mask[edge_off + poij[p]] = an; A.out_mask[edge_off + poji[p]] = an; }
         }
       }
@@ -435,8 +557,9 @@ cudaError_t with_var_kernel(int graph_mode, const GxModelDev& m, F&& f) {
   return var_dispatch(m, [&](auto bn, auto kw) {
     constexpr bool b = decltype(bn)::value;
     constexpr int w = decltype(kw)::value;
-    if (m.att) return graph_mode ? f(explain_var_kernel<true, b, w, true>) : f(explain_var_kernel<false, b, w, true>);
-    return graph_mode ? f(explain_var_kernel<true, b, w, false>) : f(explain_var_kernel<false, b, w, false>);
+    if (m.att) return graph_mode ? f(explain_var_kernel<true, b, w, true, false>) : f(explain_var_kernel<false, b, w, true, false>);
+    if (m.d >= GX_VAR_WIDE_MIN) return graph_mode ? f(explain_var_kernel<true, b, w, false, true>) : f(explain_var_kernel<false, b, w, false, true>);
+    return graph_mode ? f(explain_var_kernel<true, b, w, false, false>) : f(explain_var_kernel<false, b, w, false, false>);
   });
 }
 
@@ -445,7 +568,9 @@ cudaError_t with_var_kernel(int graph_mode, const GxModelDev& m, F&& f) {
 // var_smem's carve-up + in graph mode the edge-less rows' constant embedding and the arg-max row of every pooled feature (cst, arg)
 int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C, int att) {
   const int pool = graph_mode ? 2 * gx_round_up(hid * (L - 1) + emb, 4) : 0;
-  return (var_smem(d, L, hid, emb, C, kVarThreads / 32, att).total + pool) * 4;
+  const int words = d >= GX_VAR_WIDE_MIN ? var_smem_wide(d, L, hid, emb, C, kVarThreads / 32).total
+                                         : var_smem(d, L, hid, emb, C, kVarThreads / 32, att).total;
+  return (words + pool) * 4;
 }
 int gx_var_row_stride(int hid, int emb) { return 32 * var_kw(hid, emb); }
 

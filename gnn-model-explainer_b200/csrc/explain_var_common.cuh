@@ -58,11 +58,52 @@ __host__ __device__ inline VarSmem var_smem(int d, int L, int hid, int emb, int 
   return S;
 }
 
+// Wide inputs (d > 128, explain_var.cu kWide) keep the feature-mask state and layer 1's products in the task slab and read W1 through
+// L2, so that nothing here grows with d: no feature-mask arrays or dL/dsF partials, hidden-width scratch rows, and only the layers
+// >= 2 are staged (S.W[0] takes zero words).
+__host__ __device__ inline VarSmem var_smem_wide(int d, int L, int hid, int emb, int C, int nwarps) {
+  VarSmem S;
+  int o = 0;
+  auto take = [&](int words) { int r = o; o += gx_round_up(words, 4); return r; };
+  int wwords = 0;
+  for (int l = 1; l < L; ++l) wwords += hid * (l == L - 1 ? emb : hid);
+  S.w_in_smem = wwords <= kVarWeightWords;
+  for (int l = 0; l < L; ++l) {
+    const int wout = l == L - 1 ? emb : hid;
+    S.W[l] = take(S.w_in_smem && l > 0 ? hid * wout : 0);
+    S.b[l] = take(wout);
+  }
+  const int PD = hid * (L - 1) + emb;
+  S.Wp = take(C * (PD + 1) <= GX_WP_SMEM_MAX ? C * (PD + 1) : 0);
+  S.sF = S.F = S.mF = S.vF = o;
+  S.zlen = 32 * var_kw(hid, emb);
+  S.zs = take(nwarps * S.zlen);
+  S.gFp = o;
+  S.emb = take(PD); S.dEmb = take(PD); S.logit = take(C < 32 ? 32 : C);
+  S.total = o;
+  (void)d;
+  return S;
+}
+template <bool kWide>
+__host__ __device__ inline VarSmem var_smem_of(int d, int L, int hid, int emb, int C, int nwarps, int att) {
+  if constexpr (kWide) return var_smem_wide(d, L, hid, emb, C, nwarps);
+  else return var_smem(d, L, hid, emb, C, nwarps, att);
+}
+
 // Stages conv biases (always), conv weights (when S.w_in_smem) and pred_model (when small) in shared memory; Wl[l] = where layer l's
 // weights are read from.
+// With kWide, layer 1's weights stay in global memory (var_smem_wide).
+template <bool kWide = false>
 __device__ __forceinline__ void var_stage_model(const GxModelDev& m, const VarSmem& S, float* sm, const float** Wl, int tid, int nt) {
   const int L = m.L, PD = m.hid * (L - 1) + m.emb;
   for (int l = 0; l < L; ++l) {
+    if constexpr (kWide) {
+      if (l == 0) {
+        Wl[0] = m.W[0];
+        for (int idx = tid; idx < m.hid; idx += nt) sm[S.b[0] + idx] = __ldg(m.b[0] + idx);
+        continue;
+      }
+    }
     const int win = l == 0 ? m.d : m.hid, wout = l == L - 1 ? m.emb : m.hid;
     const int cnt = win * wout;
     if (S.w_in_smem)
@@ -179,6 +220,21 @@ __device__ __forceinline__ float var_activate(const float (&y)[KW], int wout, bo
 }
 // Layer l's per-row arrays, as the kernels' slab accessors give them: Yh(l) normalised pre-activations (row stride 32 * KW), H(l) outputs
 // (row stride ldh), qn(l) norms, istd(l) the bn standardisation's 1/std.  The addresses are formed where they are used.
+// Row i of layer l (1 .. L) from its pre-activation y: var_activate, then the stores (H is 0 in the padding lanes).  (The wide path's
+// layer 1; var_row_forward below is the same steps after y = b + zs W.)
+template <bool kBn, int KW, typename YhF, typename HF, typename QF, typename IF>
+__device__ __forceinline__ void var_row_epilogue(const float (&y)[KW], int wout, int l, int L, int i, YhF Yh, HF H, int64_t ldh, QF qn, IF istd,
+                                                 int lane) {
+  float yh[KW], h[KW], is = 1.f;
+  const float q = var_activate<kBn, KW>(y, wout, l < L, yh, h, &is, lane);
+  if (kBn && l < L && lane == 0) istd(l)[i] = is;
+#pragma unroll
+  for (int k = 0; k < KW; ++k) {
+    Yh(l)[(int64_t)i * (32 * KW) + lane + 32 * k] = yh[k];
+    H(l)[(int64_t)i * ldh + lane + 32 * k] = lane + 32 * k < wout ? h[k] : 0.f;
+  }
+  if (lane == 0) qn(l)[i] = q;
+}
 // Row i of layer l (1 .. L) after its aggregate is in zs: y = b + zs W, var_activate, then the stores (H is 0 in the padding lanes).
 template <bool kBn, int KW, typename YhF, typename HF, typename QF, typename IF>
 __device__ __forceinline__ void var_row_forward(const float* zs, int win, const float* Ws, int wout, const float* bsm, int l, int L, int i,

@@ -129,7 +129,8 @@ __global__ void __launch_bounds__(kFwdThreads) readout_kernel(int64_t N, int L, 
 
 }  // namespace
 
-// H: workspace [L][N][32] floats (device).  pred [N][C], emb_out [N][PD] or nullptr (device).  P: attention models' workspace
+// H: workspace [L][N][32] floats (device).  Layer 1 keeps one input row per warp in dynamic shared memory: 128 KB at the widest
+// input (d = 4096), beyond the 48 KB a launch gets without opting in.  pred [N][C], emb_out [N][PD] or nullptr (device).  P: attention models' workspace
 // [N][round_up(max(d, hid), 4)] floats (device), else unused.
 cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, float* pred, float* emb_out, float* P, cudaStream_t s) {
   const int nwarps = kFwdThreads / 32;
@@ -144,6 +145,10 @@ cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, fl
       if (l == 0) gcn_layer_kernel<true, true><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, P, Hout);
       else gcn_layer_kernel<false, true><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, P, Hout);
       continue;
+    }
+    if (l == 0 && smem > 48 * 1024) {
+      const cudaError_t e = cudaFuncSetAttribute(gcn_layer_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e != cudaSuccess) return e;
     }
     if (l == 0) gcn_layer_kernel<true, false><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, nullptr, Hout);
     else gcn_layer_kernel<false, false><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, nullptr, Hout);

@@ -210,21 +210,25 @@ __host__ __device__ inline GxStreamLayout gx_make_stream_layout(int n, int n1, i
 // Graph mode computes every one of its n rows with an edge at every layer (n2 = n, e1 = e_d) and has no Laplacian term (np_in = 0).
 // Attention models (att != 0, e_d = all directed slots of the task) add the per-layer projections and edge weights; for any other
 // model these arrays take zero words.
+// Wide inputs (wide != 0: d > 128) contract layer 1 as A_m (X (sigmoid(F) (.) W1)): U and dZ1 take zero words, the masked adjacency
+// covers all e_d slots (dP gathers over the rows beyond n2), and the feature-mask state and the hid-wide products P, dY1, dP and G
+// live here.  For d <= 128 these arrays take zero words.
 struct GxVarLayout {
   int64_t a, U, dZ1, lapg, Yh, H, dZ, q, istd;
   int64_t P, s, as, t, cw, dHa;
+  int64_t fm, XB, dY1, dP, G;
   int64_t total_words;
 };
 __host__ __device__ inline GxVarLayout gx_make_var_layout(int n, int n2, int e1, int np_in, int d, int L, int vw = 32, int att = 0,
-                                                          int e_d = 0) {
+                                                          int e_d = 0, int wide = 0) {
   GxVarLayout Lo;
   const int dp = gx_round_up(d, 4);
   int64_t o = 0;
   auto take = [&](int64_t words) { int64_t r = o; o += (words + 3) / 4 * 4; return r; };
   (void)n;
-  Lo.a = take(e1);                            // masked adjacency of the rows the forward visits (level-order rows < n2)
-  Lo.U = take((int64_t)n2 * dp);              // A_m X
-  Lo.dZ1 = take((int64_t)n2 * dp);            // dL/d(A_m X') (.) sigmoid(feat_mask)
+  Lo.a = take(wide ? e_d : e1);               // masked adjacency of the rows the forward visits (level-order rows < n2; wide: every row)
+  Lo.U = take(wide ? 0 : (int64_t)n2 * dp);   // A_m X
+  Lo.dZ1 = take(wide ? 0 : (int64_t)n2 * dp); // dL/d(A_m X') (.) sigmoid(feat_mask)
   Lo.lapg = take(np_in);
   Lo.Yh = take((int64_t)L * n2 * vw);         // per layer: normalised pre-activations (row stride vw = 32 * ceil(width / 32))
   Lo.H = take((int64_t)L * n2 * vw);          // per layer: relu (+ standardisation) output = input of the next layer / the readout
@@ -238,6 +242,12 @@ __host__ __device__ inline GxVarLayout gx_make_var_layout(int n, int n2, int e1,
   Lo.t = take(at * L * e1);                   // per layer and slot of a row of the layer: t_ij = dL/dZ_i . H_{l-1}[j]
   Lo.cw = take(at * e_d);                     // the current layer's a_ij (t_ij + t_ji) on every slot (rows beyond n2 included)
   Lo.dHa = take(at * n2 * vw);                // dL/dP Wa^T of the layer above: the attention's share of dL/dH
+  const int64_t wd = wide ? 1 : 0;
+  Lo.fm = take(wd * 5 * dp);                  // sigmoid(F), F, the optimiser's two moments, dL/dsigmoid(F) (dp words each)
+  Lo.XB = take(wd * n * vw);                  // P = X (sigmoid(F) (.) W1) of every row of the task
+  Lo.dY1 = take(wd * n2 * vw);                // dL/dY of layer 1's rows
+  Lo.dP = take(wd * n * vw);                  // A_m^T dY1 of every row
+  Lo.G = take(wd * dp * vw);                  // X^T dP (d, hid)
   Lo.total_words = o;
   return Lo;
 }
@@ -391,6 +401,8 @@ cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, int graph_mode, co
                                   const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                   float* out_mask, float* out_feat, cudaStream_t s);
 int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C, int att = 0);
+constexpr int GX_VAR_WIDE_MIN = 129;    // input widths from here on run the variant kernel's wide path (layer 1 contracted as A_m (X B))
+constexpr int GX_VAR_WIDE_MAX = 4096;   // the largest input width the wide path builds
 int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m);
 int gx_var_row_stride(int hid, int emb);
 // explain_dense.cu: Explainer.explain(..., unconstrained=True), node mode (graph_mode 0, g) or graph mode (gb); m0 / out_dense are dense

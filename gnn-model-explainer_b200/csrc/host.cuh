@@ -211,7 +211,7 @@ int size_slab_launch(gx_handle* h, const char* who, const std::vector<int32_t>& 
 // Words of task T's slab in explain_var.cu (graph mode has no Laplacian term, so no per-pair lapg)
 inline int64_t var_slab_words(const gx_handle* h, int graph_mode, const GxTask& T) {
   return gx_make_var_layout(T.n, T.n2, T.e1, graph_mode ? 0 : T.npairs_in, h->m.d, h->m.L, gx_var_row_stride(h->m.hid, h->m.emb), h->m.att,
-                            T.e_d).total_words;
+                            T.e_d, h->m.d >= GX_VAR_WIDE_MIN).total_words;
 }
 
 // One persistent launch of explain_var.cu over the whole plan (d_order, work-queue counter 0), each CTA with a task slab and a pair

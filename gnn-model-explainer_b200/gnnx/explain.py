@@ -106,12 +106,13 @@ class Explainer:
         self.engine = Engine(device)
         weights, num_layers = model_weights(model)
         self._att = "Wa1" in weights
+        self._wide = weights["W1"].shape[0] > 128   # inputs wider than 128: the variant kernel's wide path
         self.engine.set_model(weights, num_layers=num_layers, bn=bn,
                               att=[weights["Wa%d" % l] for l in range(1, num_layers + 1)] if self._att else None)
         if getattr(args, "gnnx_latency", False):
             self.engine.debug_cluster(0, 0)   # latency mode: thread-block clusters for the expensive tasks of batches that leave SMs idle
         # model / optimiser variants run in the variant kernel, which does not log the per-epoch trace print_training replays
-        self._no_trace = bn or num_layers != 3 or getattr(args, "opt", "adam") != "adam" or self._att
+        self._no_trace = bn or num_layers != 3 or getattr(args, "opt", "adam") != "adam" or self._att or self._wide
         adj_np = np.asarray(adj)
         if graph_mode:
             # graph classification: the whole padded batch goes to the device once (explain.py:80-85)
@@ -247,6 +248,8 @@ class Explainer:
             return plan, edge_mask
         if unconstrained and self._att:
             raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
+        if unconstrained and self._wide:
+            raise NotImplementedError("unconstrained=True is not built for inputs wider than 128 features")
         hp, init = self._hparams()
         if unconstrained:
             # explain.py:688-692: the dense mask drives the forward, so every one of the n^2 normals of M0 is a parameter
@@ -277,6 +280,8 @@ class Explainer:
     def _print_no_trace(self):
         if self._att:
             print("(per-epoch trace is not built for attention models (--method att))")
+        elif self._wide:
+            print("(per-epoch trace is not built for inputs wider than 128 features)")
         else:
             print("(per-epoch trace is not built for --bn / num_gc_layers != 3 / optimisers other than Adam)")
 
@@ -308,6 +313,8 @@ class Explainer:
     def _explain_graph_batch(self, graph_indices, unconstrained=False):
         if unconstrained and self._att:
             raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
+        if unconstrained and self._wide:
+            raise NotImplementedError("unconstrained=True is not built for inputs wider than 128 features")
         gids = [int(g) for g in graph_indices]
         edge_off = self.engine.plan_graphs(gids)
         hp, init = self._hparams()

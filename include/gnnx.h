@@ -43,7 +43,7 @@ typedef enum gx_memspace { GX_HOST = 0, GX_DEVICE = 1 } gx_memspace;
 /* Model dimensions: GcnEncoderNode/GcnEncoderGraph(input_dim, hidden_dim, embedding_dim, label_dim,
  * num_layers, bn=..., args.bias) -- reference models.py:84-97,332-345. */
 typedef struct gx_model_dims {
-  int32_t input_dim;   /* d                                             */
+  int32_t input_dim;   /* d: 1..4096.  d > 128 runs on the model-variant kernel's wide path (any layers / bn / widths; not attention models) */
   int32_t hidden_dim;  /* output width of conv_first / conv_block[*]    */
   int32_t embed_dim;   /* output width of conv_last                     */
   int32_t num_classes; /* label_dim                                     */
@@ -51,8 +51,8 @@ typedef struct gx_model_dims {
   int32_t flags;       /* GX_MODEL_* bits                               */
 } gx_model_dims;
 #define GX_MODEL_BN 1u /* args.bn (models.py:222-228): per-node standardisation after every hidden ReLU.  num_layers != 3, bn, att or
-                        * a hidden / output width of 33..128 select the model-variant kernels (node mode and graph mode, mask
-                        * optimisation only: no trace / optimiser state / grad) */
+                        * a hidden / output width of 33..128 or an input width above 128 select the model-variant kernels (node mode
+                        * and graph mode, mask optimisation only: no trace / optimiser state / grad / unconstrained masks for d > 128) */
 #define GX_MODEL_ATT 2u /* args.method == "att" (models.py:62-68): every layer scales the adjacency by s_ij = P_i . P_j, P = H Wa.
                          * Set by gx_set_model_att only (gx_set_model refuses it: the attention weights arrive with that call). */
 

@@ -2,7 +2,8 @@
 """Small invocation of every kernel for compute-sanitizer (racecheck / memcheck / synccheck are ~100x slower than a plain run):
     compute-sanitizer --tool racecheck python tools/sanitize_run.py
 k-hop extraction + shared-memory kernel on a mix of task sizes (syn1: hub node 0 and tiny tasks), the streaming kernel (forced),
-the gradient baseline, graph mode, densify, neighbourhood rows, the unconstrained (dense) kernel, attention models.  A few epochs each."""
+the gradient baseline, graph mode, densify, neighbourhood rows, the unconstrained (dense) kernel, attention models, inputs wider than 128
+features (explain_var.cu's wide path).  A few epochs each."""
 import os
 import sys
 
@@ -19,7 +20,7 @@ EPOCHS = int(os.environ.get("SAN_EPOCHS", "4"))
 
 
 def main():
-    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster", "dense", "att"]
+    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster", "dense", "att", "wide"]
     fx = util.load_fixture("syn1")
     if "node" in which:
         eng = util.make_engine(fx)
@@ -171,6 +172,52 @@ def main():
         out = np.zeros(int(eoff[-1]), np.float32)
         eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=9), None, out)
         print("att ok graph", float(out.sum()))
+        eng.close()
+    if "wide" in which:   # explain_var.cu's wide path (d > 128): node mode with the hub and small tasks (rows beyond n2 gather dP), a
+        # --bn 4-layer model with width 128, graph mode with one-hot features, and the model forward at d = 1500 (> 48 KB of shared memory)
+        rng = np.random.default_rng(11)
+        d0, C0 = 300, fx.weights["Wp"].shape[0]
+        feat = rng.normal(size=(fx.N, d0)).astype(np.float32)
+        for hid, L, bn in ((20, 3, False), (128, 4, True)):
+            dims = [d0] + [hid] * L
+            w = {}
+            for l in range(1, L + 1):
+                w["W%d" % l] = (rng.normal(size=(dims[l - 1], dims[l])) / np.sqrt(dims[l - 1])).astype(np.float32)
+                w["b%d" % l] = (rng.normal(size=dims[l]) * 0.3).astype(np.float32)
+            w["Wp"] = (rng.normal(size=(C0, hid * L)) * 0.3).astype(np.float32); w["bp"] = np.zeros(C0, np.float32)
+            eng = gnnx.Engine(0)
+            eng.set_model(w, num_layers=L, bn=bn)
+            eng.set_graph_csr(fx.rowptr, fx.col, feat, fx.label, fx.pred_label)
+            plan = eng.plan_nodes([0, 300, 5, 683], L)
+            out = np.zeros(plan.total_edges, np.float32)
+            fm = np.zeros((plan.count, d0), np.float32)
+            eng.explain_nodes_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=8, opt=0 if bn else 1), None, out, fm)
+            pred = eng.model_forward() if hid <= 32 else np.zeros(1)
+            print("wide ok node", hid, L, bn, float(out.sum()), float(fm.sum()), float(pred.sum()))
+            eng.close()
+        g = np.load(util.GOLDEN + "/graphs_golden.npz")
+        dg, Cg = 190, g["Wp"].shape[0]
+        adj = g["adj"]
+        featg = (np.eye(dg, dtype=np.float32)[rng.integers(0, dg, size=adj.shape[:2])] * (adj.sum(2, keepdims=True) > 0)).astype(np.float32)
+        w = dict(W1=(rng.normal(size=(dg, 20)) / np.sqrt(dg)).astype(np.float32), b1=np.ones(20, np.float32) * 0.1,
+                 W2=(rng.normal(size=(20, 20)) * 0.3).astype(np.float32), b2=np.zeros(20, np.float32),
+                 W3=(rng.normal(size=(20, 20)) * 0.3).astype(np.float32), b3=np.zeros(20, np.float32),
+                 Wp=(rng.normal(size=(Cg, 60)) * 0.3).astype(np.float32), bp=np.zeros(Cg, np.float32))
+        eng = gnnx.Engine(0)
+        eng.set_model(w, num_layers=3)
+        eng.set_graph_batch(adj, featg, g["label"])
+        eoff = eng.plan_graphs([0, 3, 5, 11])
+        out = np.zeros(int(eoff[-1]), np.float32)
+        eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=9), None, out)
+        print("wide ok graph", float(out.sum()))
+        eng.close()
+        w = dict(W1=(rng.normal(size=(1500, 20)) / np.sqrt(1500)).astype(np.float32), b1=np.zeros(20, np.float32),
+                 W2=(rng.normal(size=(20, 20)) * 0.3).astype(np.float32), b2=np.zeros(20, np.float32),
+                 Wp=(rng.normal(size=(C0, 40)) * 0.3).astype(np.float32), bp=np.zeros(C0, np.float32))
+        eng = gnnx.Engine(0)
+        eng.set_model(w, num_layers=2)
+        eng.set_graph_csr(fx.rowptr, fx.col, rng.normal(size=(fx.N, 1500)).astype(np.float32), fx.label, fx.pred_label)
+        print("wide ok forward", float(eng.model_forward().sum()))
         eng.close()
     if "misc" in which:
         eng = util.make_engine(fx)
