@@ -284,6 +284,42 @@ static int check_model_dims(const char* who, const gx_model_dims* dims) {
   return GX_OK;
 }
 
+// gx_offedge_regularisers (graph = false, after gx_plan_nodes: one n_t x n_t block per node) and gx_offedge_regularisers_graphs
+// (graph = true, after gx_plan_graphs: one max_nodes x max_nodes block per graph).
+static int offedge_impl(gx_handle* h, bool graph, const gx_hparams* hp, gx_memspace space, const float* m0_dense, double* out) {
+  const char* who = graph ? "gx_offedge_regularisers_graphs" : "gx_offedge_regularisers";
+  if (!h || !hp || !m0_dense || !out) { gx_set_error("%s: NULL argument", who); return GX_ERR_INVALID; }
+  if (graph ? !h->has_gplan : !h->has_plan) { gx_set_error("%s: no plan (call %s)", who, graph ? "gx_plan_graphs" : "gx_plan_nodes"); return GX_ERR_INVALID; }
+  if (hp->num_epochs < 1 || hp->num_epochs > 3072) { gx_set_error("%s: num_epochs outside [1,3072]", who); return GX_ERR_INVALID; }
+  GX_CUDA_CHECK(cudaSetDevice(h->device));
+  const int count = h->count, E = hp->num_epochs;
+  int64_t dense = (int64_t)count * h->gb.max_nodes * h->gb.max_nodes;
+  int rc = graph ? GX_OK : upload_dense_offsets(h, &dense);
+  if (rc != GX_OK) return rc;
+  GxHparamsDev hd;
+  fill_hparams(h, hp, 0, false, &hd);
+  if (hp->opt != GX_OPT_ADAM) { gx_set_error("%s: the off-edge trajectories are built for Adam only", who); return GX_ERR_UNSUPPORTED; }
+  rc = check_optimiser(who, hp);
+  if (rc != GX_OK) return rc;
+  rc = upload_adam_table(h, hp, E, 0);
+  if (rc != GX_OK) return rc;
+  hd.adam_tab = h->d_adam.as<float2>();
+  const float* m0d = m0_dense;
+  double* od = out;
+  const size_t nout = (size_t)count * E * 2;
+  if (space == GX_HOST) {
+    GX_CUDA_CHECK(stage_in(h, h->d_m0dense, m0_dense, (size_t)dense, &m0d));
+    GX_CUDA_CHECK(stage_out(h->d_offedge, out, nout, &od));
+  }
+  GX_CUDA_CHECK(cudaMemsetAsync(od, 0, nout * 8, h->stream));
+  if (graph) GX_CUDA_CHECK(gx_launch_offedge_graphs(hd, h->plan, h->gb, count, E, m0d, od, h->stream));
+  else GX_CUDA_CHECK(gx_launch_offedge(hd, h->plan, count, E, h->d_dense_off.as<int64_t>(), m0d, od, h->stream));
+  h->launches += 1;
+  if (space == GX_HOST) GX_CUDA_CHECK(stage_back(h, out, (const double*)od, nout));
+  GX_CUDA_CHECK(cudaStreamSynchronize(h->stream));
+  return GX_OK;
+}
+
 extern "C" {
 
 const char* gx_last_error(void) { return g_err; }
@@ -562,35 +598,11 @@ int gx_set_graph_csr(gx_handle* h, int64_t N, const int32_t* rowptr, const int32
 }
 
 int gx_offedge_regularisers(gx_handle* h, const gx_hparams* hp, gx_memspace space, const float* m0_dense, double* out) {
-  if (!h || !hp || !m0_dense || !out) { gx_set_error("gx_offedge_regularisers: NULL argument"); return GX_ERR_INVALID; }
-  if (!h->has_plan) { gx_set_error("gx_offedge_regularisers: no plan (call gx_plan_nodes)"); return GX_ERR_INVALID; }
-  if (hp->num_epochs < 1 || hp->num_epochs > 3072) { gx_set_error("gx_offedge_regularisers: num_epochs outside [1,3072]"); return GX_ERR_INVALID; }
-  GX_CUDA_CHECK(cudaSetDevice(h->device));
-  const int count = h->count, E = hp->num_epochs;
-  int64_t dense = 0;
-  int rc = upload_dense_offsets(h, &dense);
-  if (rc != GX_OK) return rc;
-  GxHparamsDev hd;
-  fill_hparams(h, hp, 0, false, &hd);
-  if (hp->opt != GX_OPT_ADAM) { gx_set_error("gx_offedge_regularisers: the off-edge trajectories are built for Adam only"); return GX_ERR_UNSUPPORTED; }
-  rc = check_optimiser("gx_offedge_regularisers", hp);
-  if (rc != GX_OK) return rc;
-  rc = upload_adam_table(h, hp, E, 0);
-  if (rc != GX_OK) return rc;
-  hd.adam_tab = h->d_adam.as<float2>();
-  const float* m0d = m0_dense;
-  double* od = out;
-  const size_t nout = (size_t)count * E * 2;
-  if (space == GX_HOST) {
-    GX_CUDA_CHECK(stage_in(h, h->d_m0dense, m0_dense, (size_t)dense, &m0d));
-    GX_CUDA_CHECK(stage_out(h->d_offedge, out, nout, &od));
-  }
-  GX_CUDA_CHECK(cudaMemsetAsync(od, 0, nout * 8, h->stream));
-  GX_CUDA_CHECK(gx_launch_offedge(hd, h->plan, count, E, h->d_dense_off.as<int64_t>(), m0d, od, h->stream));
-  h->launches += 1;
-  if (space == GX_HOST) GX_CUDA_CHECK(stage_back(h, out, (const double*)od, nout));
-  GX_CUDA_CHECK(cudaStreamSynchronize(h->stream));
-  return GX_OK;
+  return offedge_impl(h, false, hp, space, m0_dense, out);
+}
+
+int gx_offedge_regularisers_graphs(gx_handle* h, const gx_hparams* hp, gx_memspace space, const float* m0_dense, double* out) {
+  return offedge_impl(h, true, hp, space, m0_dense, out);
 }
 
 int gx_comm_unique_id(char id[128]) {

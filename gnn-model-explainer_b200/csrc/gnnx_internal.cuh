@@ -438,5 +438,7 @@ cudaError_t gx_launch_unshard(const float* gathered, int items, const int64_t* s
 cudaError_t gx_launch_trace_finalize(const GxHparamsDev& hp, const GxPlanArrays& plan, int count, const GxExtra& x, cudaStream_t s);
 cudaError_t gx_launch_offedge(const GxHparamsDev& hp, const GxPlanArrays& plan, int count, int epochs, const int64_t* dense_off,
                               const float* m0_dense, double* out, cudaStream_t s);
+cudaError_t gx_launch_offedge_graphs(const GxHparamsDev& hp, const GxPlanArrays& plan, const GxGraphBatchDev& gb, int count, int epochs,
+                                     const float* m0_dense, double* out, cudaStream_t s);
 cudaError_t gx_launch_densify(const GxPlanArrays& plan, int count, const int64_t* dense_off,
                               const float* edge_mask, double* out, cudaStream_t s);

@@ -218,6 +218,7 @@ class Engine:
         edge_off = np.empty(len(gids) + 1, np.int64)
         te = C.c_int64()
         _abi.check(self._lib.gx_plan_graphs(self._h, _np_ptr(gids), len(gids), _np_ptr(edge_off), C.byref(te)))
+        self._graph_count = len(gids)
         return edge_off
 
     def graph_rows_cols(self, g):
@@ -287,6 +288,16 @@ class Engine:
         out = np.zeros((count, hp.num_epochs, 2), np.float64)
         m0_dense = _f32c(m0_dense)
         _abi.check(self._lib.gx_offedge_regularisers(self._h, C.byref(hp), _abi.GX_HOST, _np_ptr(m0_dense), _np_ptr(out)))
+        return out
+
+    def offedge_regularisers_graphs(self, hp, m0_dense):
+        """The same for the planned graphs (gx_offedge_regularisers_graphs): m0_dense = the (max_nodes, max_nodes) M0 of every
+        planned graph in plan order; the sums run over all entries but the graph's directed edges (padded rows, non-edges, diagonal)."""
+        out = np.zeros((self._graph_count, hp.num_epochs, 2), np.float64)
+        m0_dense = _f32c(m0_dense)
+        if m0_dense.size != self._graph_count * self.batch_n * self.batch_n:
+            raise ValueError("m0_dense has %d entries, expected %d graphs x %d^2" % (m0_dense.size, self._graph_count, self.batch_n))
+        _abi.check(self._lib.gx_offedge_regularisers_graphs(self._h, C.byref(hp), _abi.GX_HOST, _np_ptr(m0_dense), _np_ptr(out)))
         return out
 
     def grad_nodes_host(self, edge_mask_out):

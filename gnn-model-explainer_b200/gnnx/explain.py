@@ -111,8 +111,12 @@ class Explainer:
                               att=[weights["Wa%d" % l] for l in range(1, num_layers + 1)] if self._att else None)
         if getattr(args, "gnnx_latency", False):
             self.engine.debug_cluster(0, 0)   # latency mode: thread-block clusters for the expensive tasks of batches that leave SMs idle
-        # model / optimiser variants run in the variant kernel, which does not log the per-epoch trace print_training replays
-        self._no_trace = bn or num_layers != 3 or getattr(args, "opt", "adam") != "adam" or self._att or self._wide
+        # model / optimiser variants run in the variant kernel, which does not log the per-epoch trace print_training replays: the
+        # selection of gx_set_model (--bn, num_gc_layers != 3, hidden or output widths above 32, inputs wider than 128, attention)
+        # and every optimiser other than Adam
+        self._wide_layers = max(weights["W%d" % l].shape[1] for l in range(1, num_layers + 1)) > 32
+        self._no_trace = (bn or num_layers != 3 or self._wide_layers or getattr(args, "opt", "adam") != "adam" or self._att
+                          or self._wide)
         adj_np = np.asarray(adj)
         if graph_mode:
             # graph classification: the whole padded batch goes to the device once (explain.py:80-85)
@@ -260,7 +264,7 @@ class Explainer:
             trace = np.zeros((plan.count, hp.num_epochs, _abi.GX_TRACE_COLS), np.float32)
             pred = np.zeros((plan.count, hp.num_epochs, self.engine.num_classes), np.float32)
             self.engine.explain_nodes_unconstrained(hp, m0, edge_mask, trace=trace, trace_pred=pred)
-            self.last_trace = self._print_trace(plan, hp, trace, pred, None)    # the kernel's loss covers all n^2 entries
+            self.last_trace = self._print_trace(hp, trace, pred, None, None)    # the kernel's loss covers all n^2 entries
             return plan, edge_mask
         if not self.print_training or self._no_trace:
             if self.print_training:
@@ -274,7 +278,7 @@ class Explainer:
         pred = np.zeros((plan.count, hp.num_epochs, self.engine.num_classes), np.float32)
         self.engine.explain_nodes_ex(hp, m0, edge_mask, trace=trace, trace_pred=pred)
         off = self.engine.offedge_regularisers(hp, np.concatenate([D.reshape(-1) for D in dense])) if dense is not None else None
-        self.last_trace = self._print_trace(plan, hp, trace, pred, off)
+        self.last_trace = self._print_trace(hp, trace, pred, off, np.diff(plan.node_off).astype(np.float64) ** 2)
         return plan, edge_mask
 
     def _print_no_trace(self):
@@ -283,18 +287,18 @@ class Explainer:
         elif self._wide:
             print("(per-epoch trace is not built for inputs wider than 128 features)")
         else:
-            print("(per-epoch trace is not built for --bn / num_gc_layers != 3 / optimisers other than Adam)")
+            print("(per-epoch trace is not built for --bn / num_gc_layers != 3 / optimisers other than Adam / hidden or output widths above 32)")
 
-    def _print_trace(self, plan, hp, trace, pred, off):
-        """Replays the reference's per-epoch print (explain.py:148-159).  With the torch-compatible init the loss is the
-        reference's own number (edge part from the kernels + the regulariser sums over the n^2 - E_d mask entries that never reach
-        the result, gx_offedge_regularisers); with the device init those entries are never materialised and the printed loss
-        covers the edge entries only."""
+    def _print_trace(self, hp, trace, pred, off, nn):
+        """Replays the reference's per-epoch print (explain.py:148-159), task after task.  With the torch-compatible init the loss is
+        the reference's own number (edge part from the kernels + the regulariser sums over the n^2 - E_d mask entries that never reach
+        the result, gx_offedge_regularisers / gx_offedge_regularisers_graphs; nn[t] = n^2 of task t's dense mask: the k-hop set in node
+        mode, max_nodes in graph mode); with the device init those entries are never materialised and the printed loss covers the
+        edge entries only."""
         loss = trace[:, :, _abi.TR_LOSS_EDGES].astype(np.float64)
         if off is not None:
-            nn = np.diff(plan.node_off).astype(np.float64)[:, None] ** 2
-            loss = loss + hp.coef_size * off[:, :, 0] + hp.coef_ent * off[:, :, 1] / nn
-        for t in range(plan.count):
+            loss = loss + hp.coef_size * off[:, :, 0] + hp.coef_ent * off[:, :, 1] / np.asarray(nn, np.float64)[:, None]
+        for t in range(trace.shape[0]):
             for epoch in range(hp.num_epochs):
                 print("epoch: ", epoch, "; loss: ", float(loss[t, epoch]), "; mask density: ", float(trace[t, epoch, _abi.TR_DENSITY]),
                       "; pred: ", torch.from_numpy(pred[t, epoch]))
@@ -310,6 +314,9 @@ class Explainer:
         return fname
 
     # ---------------------------------------------------------------- public API
+    # a trace is built for at most this many epochs per call (gx_explain_io.trace); longer runs print a notice instead
+    _MAX_TRACE_EPOCHS = 1536
+
     def _explain_graph_batch(self, graph_indices, unconstrained=False):
         if unconstrained and self._att:
             raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
@@ -318,25 +325,48 @@ class Explainer:
         gids = [int(g) for g in graph_indices]
         edge_off = self.engine.plan_graphs(gids)
         hp, init = self._hparams()
-        if self.print_training and self._no_trace and not unconstrained:
-            self._print_no_trace()
+        # print_training (explain.py:148-159): the kernels log every epoch; the unconstrained kernel for every model, the tuned kernel
+        # for the default model with Adam, up to _MAX_TRACE_EPOCHS epochs
+        traced = self.print_training and (unconstrained or (not self._no_trace and hp.num_epochs <= self._MAX_TRACE_EPOCHS))
+        if self.print_training and not traced:
+            if self._no_trace:
+                self._print_no_trace()
+            else:
+                print("(per-epoch trace is not built for more than %d epochs per call)" % self._MAX_TRACE_EPOCHS)
         n = self.engine.batch_n
         m0 = None
+        dense = None      # the full (n, n) draws: the unconstrained kernel's M0, or the off-edge entries of the printed loss
         rc = [self.engine.graph_rows_cols(g) for g in gids]
         if init == "torch":
-            m0 = np.empty(n * n * len(gids) if unconstrained else int(edge_off[-1]), dtype=np.float32)
+            if unconstrained or traced:
+                dense = np.empty(n * n * len(gids), dtype=np.float32)
+            if not unconstrained:
+                m0 = np.empty(int(edge_off[-1]), dtype=np.float32)
             std = torch.nn.init.calculate_gain("relu") * math.sqrt(2.0 / (n + n))
             for t, (rows, cols) in enumerate(rc):
                 M = torch.FloatTensor(n, n).normal_(1.0, std).numpy()      # explain.py:645-652, n = padded size
-                if unconstrained:
-                    m0[t * n * n:(t + 1) * n * n] = M.reshape(-1)
-                else:
+                if dense is not None:
+                    dense[t * n * n:(t + 1) * n * n] = M.reshape(-1)
+                if m0 is not None:
                     m0[edge_off[t]:edge_off[t + 1]] = M[rows, cols]
+            if unconstrained:
+                m0 = dense
         edge_mask = np.empty(int(edge_off[-1]), dtype=np.float32)
+        trace = pred = None
+        if traced:
+            trace = np.zeros((len(gids), hp.num_epochs, _abi.GX_TRACE_COLS), np.float32)
+            pred = np.zeros((len(gids), hp.num_epochs, self.engine.num_classes), np.float32)
         if unconstrained:
-            self.engine.explain_graphs_unconstrained(hp, m0, edge_mask)
+            self.engine.explain_graphs_unconstrained(hp, m0, edge_mask, trace=trace, trace_pred=pred)
+        elif traced:
+            self.engine.explain_nodes_ex(hp, m0, edge_mask, trace=trace, trace_pred=pred, graphs=True)
         else:
             self.engine.explain_graphs_host(hp, m0, edge_mask)
+        if traced:
+            off = None
+            if not unconstrained and dense is not None:   # the unconstrained kernel's loss already covers all n^2 entries
+                off = self.engine.offedge_regularisers_graphs(hp, dense)
+            self.last_trace = self._print_trace(hp, trace, pred, off, np.full(len(gids), float(n) * n))
         out = []
         for t, (rows, cols) in enumerate(rc):
             D = np.zeros((n, n), dtype=np.float64)

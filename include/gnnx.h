@@ -92,7 +92,8 @@ typedef struct gx_hparams {
 /* Per-epoch log of the optimisation, one row per epoch of this call (explain.py:137-159: the values print_training
  * prints, plus the terms they are made of).  "edges" = restricted to the E_d directed-edge entries of the mask; the
  * reference's printed loss also sums size/entropy over the n^2 - E_d entries that never reach the result:
- * gx_offedge_regularisers returns that remainder so that loss = GX_TR_LOSS_EDGES + c_size*S_off + c_ent*H_off/n^2. */
+ * gx_offedge_regularisers (node mode) and gx_offedge_regularisers_graphs (graph mode, n = max_nodes) return that remainder
+ * so that loss = GX_TR_LOSS_EDGES + c_size*S_off + c_ent*H_off/n^2. */
 #define GX_TRACE_COLS 8
 #define GX_TR_LOSS_EDGES 0 /* pred + size(edges) + lap + ent(edges) + feat_size  (explain.py:808)      */
 #define GX_TR_PRED 1       /* -log softmax(logits[node])[label]                  (explain.py:750-753)  */
@@ -201,6 +202,13 @@ int gx_explain_nodes_ex(gx_handle* h, const gx_hparams* hp, gx_memspace space, c
  * planned node, task after task (sum_t n_t^2 floats, `space`); out[count*num_epochs*2] = per epoch (sum sigmoid(M),
  * sum H(sigmoid(M))) over those entries, in double.  Only needed to reproduce the reference's printed loss value. */
 int gx_offedge_regularisers(gx_handle* h, const gx_hparams* hp, gx_memspace space, const float* m0_dense, double* out);
+/* The same for the planned graphs of graph mode (after gx_plan_graphs): every graph's mask is the padded max_nodes x max_nodes
+ * matrix, and the entries summed are all of them but the graph's directed edges -- padded rows and columns, non-edges and the
+ * diagonal.  m0_dense = the full (max_nodes, max_nodes) M0 of every planned graph, in plan order (count*max_nodes^2 floats,
+ * `space`); out[count*num_epochs*2] as above.  The printed loss of graph t at epoch e (explain.py:148-159, lap_loss = 0) is
+ *   GX_TR_LOSS_EDGES + c_size*out[t][e][0] + c_ent*out[t][e][1] / max_nodes^2.
+ * Both calls: Adam only (GX_ERR_UNSUPPORTED otherwise), num_epochs in [1, 3072], GX_ERR_INVALID without the matching plan. */
+int gx_offedge_regularisers_graphs(gx_handle* h, const gx_hparams* hp, gx_memspace space, const float* m0_dense, double* out);
 
 /* The gradient baseline, Explainer.explain(..., model="grad") (explain.py:125-133) with ExplainModule.adj_feat_grad
  * (explain.py:717-738), for every planned node: one forward of the frozen model on the unmasked sub-adjacency and

@@ -2,7 +2,7 @@
 """Small invocation of every kernel for compute-sanitizer (racecheck / memcheck / synccheck are ~100x slower than a plain run):
     compute-sanitizer --tool racecheck python tools/sanitize_run.py
 k-hop extraction + shared-memory kernel on a mix of task sizes (syn1: hub node 0 and tiny tasks), the streaming kernel (forced),
-the gradient baseline, graph mode, densify, neighbourhood rows, the unconstrained (dense) kernel, attention models, inputs wider than 128
+the gradient baseline, graph mode, densify, the off-edge regulariser sums of graph mode, neighbourhood rows, the unconstrained (dense) kernel, attention models, inputs wider than 128
 features (explain_var.cu's wide path).  A few epochs each."""
 import os
 import sys
@@ -227,6 +227,17 @@ def main():
         eng.explain_nodes_host(eng.make_hparams(num_epochs=2), util.golden_m0(fx, plan), out)
         dense = eng.densify_host(out, int(sum(plan.n(t) ** 2 for t in range(plan.count))))
         print("misc ok", int(rows.sum()), float(dense.sum()))
+        eng.close()
+        # the off-edge regulariser sums of graph mode (trace.cu offedge_graph_kernel): padded graphs, some with padded rows
+        g = np.load(util.GOLDEN + "/graphs_golden.npz")
+        eng = gnnx.Engine(0)
+        eng.set_model({k: g[k] for k in util.WKEYS})
+        eng.set_graph_batch(g["adj"], g["feat"], g["label"])
+        eng.plan_graphs([0, 3, 5, 11])
+        n = int(g["max_nodes"])
+        off = eng.offedge_regularisers_graphs(eng.make_hparams(num_epochs=EPOCHS),
+                                              np.random.default_rng(0).normal(1.0, 0.2, 4 * n * n).astype(np.float32))
+        print("misc ok offedge graphs", float(off.sum()))
         eng.close()
 
 
