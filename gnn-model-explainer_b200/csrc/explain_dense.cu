@@ -151,7 +151,8 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
     const GxTask* __restrict__ Tp = A.plan.tasks + task_id;
     const int n = graph ? A.gb.max_nodes : Tp->n;
     const int r = graph ? 0 : Tp->idx_new;
-    const int gt = Tp->gt_label, key = Tp->node, e_d = Tp->e_d;
+    const int gt = Tp->gt_label, key = Tp->node;
+    const int adj_sum = Tp->e_d + Tp->loops;   // sum(adj) of mask_density (explain.py:680-683): self loops count, their mask entry is 0
     const int64_t nn64 = (int64_t)n * n;
     const GxDenseLayout Lo = gx_make_dense_layout(n, d, L, VW);
     const int KH = Lo.kh, ZW = Lo.zw;
@@ -336,7 +337,7 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
             const float feat = (float)((double)hp.c_feat_size * tr[3] / (double)d);
             row[GX_TR_LOSS_EDGES] = pred + size + lap + ent + feat;
             row[GX_TR_PRED] = pred; row[GX_TR_SIZE] = size; row[GX_TR_ENT] = ent; row[GX_TR_LAP] = lap; row[GX_TR_FEAT] = feat;
-            row[GX_TR_DENSITY] = e_d > 0 ? (float)(dens[0] / (double)e_d) : 0.f;
+            row[GX_TR_DENSITY] = adj_sum > 0 ? (float)(dens[0] / (double)adj_sum) : 0.f;
             row[GX_TR_PGT] = s_pgt;
           }
         }

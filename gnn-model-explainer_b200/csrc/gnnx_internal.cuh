@@ -28,6 +28,7 @@ struct GxTask {
   int32_t status;   // 0 ok; 1 node not inside its own neighbourhood
   int32_t n_norm;   // the n of the reference's dense tensors (1/n^2 factors, M0 std): n in node mode, max_nodes in graph mode
   int32_t flags;    // graph mode: bit 0 = some row of the padded graph has no edge (its constant embedding joins the max-pool)
+  int32_t loops;    // node mode: members with a self loop (the diagonal of the reference's sub_adj; not among the e_d entries)
   int32_t cum[GX_MAX_LEVELS + 1];  // cum[t] = #nodes with dist <= t (dist measured from `node`)
   int32_t smem_bytes;              // shared-memory footprint of this task in the explainer kernel
   int64_t node_off;  // into nbrs / lo2gid

@@ -154,21 +154,21 @@ khop_count_kernel(GxGraphDev g, const int32_t* __restrict__ nodes, int count, in
                   GxSlotWs ws, GxTask* __restrict__ tasks) {
   __shared__ int s_ctrl[3];
   __shared__ int s_cnt[GX_MAX_LEVELS + 1];
-  __shared__ int s_e[3];
+  __shared__ int s_e[4];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
   const Slot sl = slot_of(ws, blockIdx.x, g.N);
   for (int t = blockIdx.x; t < count; t += gridDim.x) {
     const int root = nodes[t];
     const int tail = bfs_khop(g, root, k, sl, s_ctrl);
     if (tid <= GX_MAX_LEVELS) s_cnt[tid] = 0;
-    if (tid < 3) s_e[tid] = 0;
+    if (tid < 4) s_e[tid] = 0;
     __syncthreads();
     for (int idx0 = 1 + warp * KH_GPW; idx0 < tail; idx0 += nwarps * KH_GPW) {
       const int idx = idx0 + lane / KH_GL;
       const bool valid = idx < tail;
       const int u = valid ? sl.q[idx] : root;
       const int du = (u == root) ? 0 : (int)sl.dist[u];
-      int cnt = 0, cnt_out = 0;
+      int cnt = 0, cnt_out = 0, loop = 0;
       if (valid) {
         const int e1 = g.rowptr[u + 1];
         for (int e = g.rowptr[u] + lane % KH_GL; e < e1; e += KH_GL) {
@@ -178,13 +178,16 @@ khop_count_kernel(GxGraphDev g, const int32_t* __restrict__ nodes, int count, in
             const int dv = (v == root) ? 0 : (int)sl.dist[v];
             cnt_out += dv > row_lvl ? 1 : 0;
           }
+          loop += v == u ? 1 : 0;
         }
       }
       cnt = group_sum_i(cnt);
       cnt_out = group_sum_i(cnt_out);
+      loop = group_sum_i(loop);
       if (valid && lane % KH_GL == 0) {
         atomicAdd(&s_cnt[du], 1);
         atomicAdd(&s_e[0], cnt);
+        if (loop) atomicAdd(&s_e[3], 1);
         if (du <= row_lvl) { atomicAdd(&s_e[1], cnt); atomicAdd(&s_e[2], cnt_out); }
       }
     }
@@ -210,6 +213,7 @@ khop_count_kernel(GxGraphDev g, const int32_t* __restrict__ nodes, int count, in
       T.smem_bytes = 0;
       T.n_norm = tail - 1;
       T.flags = 0;
+      T.loops = s_e[3];
       T.node_off = T.edge_off = T.pair_off = T.rp_off = 0;
       tasks[t] = T;
     }

@@ -456,6 +456,17 @@ int gx_explain_nodes_ex(gx_handle* h, const gx_hparams* hp, gx_memspace space, c
 }
 
 int gx_grad_nodes(gx_handle* h, gx_memspace space, float* edge_mask) {
+  if (h && h->has_plan) {
+    // The reference differentiates its raw sub_adj, diagonal included: a self loop adds a term to the forward and backward and a
+    // diagonal entry sigmoid(2|g_ii|) to the result.  The kernels work on the edge list without the diagonal, so refuse.
+    for (int t = 0; t < h->count; ++t) {
+      if (h->tasks[t].loops > 0) {
+        gx_set_error("gx_grad_nodes: the neighbourhood of node %d has %d self loop(s); the gradient baseline is not built for self loops",
+                     h->tasks[t].node, h->tasks[t].loops);
+        return GX_ERR_UNSUPPORTED;
+      }
+    }
+  }
   gx_hparams hp;
   gx_default_hparams(&hp);
   gx_explain_io io;

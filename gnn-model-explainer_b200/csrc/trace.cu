@@ -33,7 +33,9 @@ trace_finalize_kernel(const GxHparamsDev hp, const GxPlanArrays plan, int count,
     const float size = (float)((double)hp.c_size * ((double)sS + oS));
     const float ent = (float)((double)hp.c_ent * ((double)sH + oH) / nn);
     const float lap = (float)((double)hp.c_lap * ((double)sL + oL) / nn);
-    const float dens = T->e_d > 0 ? (float)(((double)sD + oD) / (double)T->e_d) : 0.f;
+    // mask_density (explain.py:680-683) divides by sum(adj): the self loops count there, the masked diagonal contributes nothing
+    const int adj_sum = T->e_d + T->loops;
+    const float dens = adj_sum > 0 ? (float)(((double)sD + oD) / (double)adj_sum) : 0.f;
     row[GX_TR_LOSS_EDGES] = pred + size + lap + ent + feat;   // explain.py:808, the sums restricted to the edge entries
     row[GX_TR_PRED] = pred; row[GX_TR_SIZE] = size; row[GX_TR_ENT] = ent; row[GX_TR_LAP] = lap;
     row[GX_TR_FEAT] = feat; row[GX_TR_DENSITY] = dens; row[GX_TR_PGT] = pgt;

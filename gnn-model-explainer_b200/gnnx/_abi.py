@@ -7,6 +7,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("GNNX_LIB_PATH") or os.path.join(_HERE, "lib", "libgnnx.so")   # GNNX_LIB_PATH: tools/ A-B builds of the same ABI
 
 GX_OK = 0
+GX_ERR_UNSUPPORTED = -3    # gx_status: valid in the reference but not built here
 GX_HOST, GX_DEVICE = 0, 1
 GX_INIT_M0, GX_INIT_PHILOX, GX_INIT_STATE = 0, 1, 2
 GX_VERSION = 211

@@ -245,10 +245,15 @@ class Explainer:
         nodes = [int(i) for i in node_indices]
         plan = self.engine.plan_nodes(nodes, self.n_hops)
         edge_mask = np.empty(plan.total_edges, dtype=np.float32)
-        if model == "grad":        # explain.py:125-133: one backward to the adjacency, no mask parameters (the reference still
-            if self._hparams()[1] == "torch":      # constructs an ExplainModule per node, i.e. consumes n^2 normals: keep the RNG in step)
-                self._draw_m0(plan)
-            self.engine.grad_nodes_host(edge_mask)     # (unconstrained is ignored here, as in the reference)
+        if model == "grad":        # explain.py:125-133: one backward to the adjacency, no mask parameters
+            try:
+                self.engine.grad_nodes_host(edge_mask)     # (unconstrained is ignored here, as in the reference)
+            except _abi.GnnxError as e:
+                if e.status == _abi.GX_ERR_UNSUPPORTED:    # a neighbourhood with self loops: refused before any RNG is consumed
+                    raise NotImplementedError(str(e)) from None
+                raise
+            if self._hparams()[1] == "torch":      # the reference still constructs an ExplainModule per node, i.e. consumes n^2 normals:
+                self._draw_m0(plan)                # keep the RNG in step
             return plan, edge_mask
         if unconstrained and self._att:
             raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")

@@ -213,7 +213,9 @@ int gx_offedge_regularisers_graphs(gx_handle* h, const gx_hparams* hp, gx_memspa
 /* The gradient baseline, Explainer.explain(..., model="grad") (explain.py:125-133) with ExplainModule.adj_feat_grad
  * (explain.py:717-738), for every planned node: one forward of the frozen model on the unmasked sub-adjacency and
  * features, loss = -log softmax(logits[node])[predicted label of the node], one backward to the adjacency;
- *   edge_mask [total_edges] float32 in `space`: sigmoid(|dL/dA_ij| + |dL/dA_ji|) at the sub_col slots. */
+ *   edge_mask [total_edges] float32 in `space`: sigmoid(|dL/dA_ij| + |dL/dA_ji|) at the sub_col slots.
+ * GX_ERR_UNSUPPORTED (the message names the node) when some planned neighbourhood contains a node with a self loop: the
+ * reference differentiates its raw sub_adj, diagonal included, and returns a diagonal entry the sub_col slots have no room for. */
 int gx_grad_nodes(gx_handle* h, gx_memspace space, float* edge_mask);
 
 /* ---- graph-classification mode (Explainer(..., graph_mode=True), explain_graphs: explain.py:80-85,356-363) ----

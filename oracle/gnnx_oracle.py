@@ -331,22 +331,77 @@ def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
 # ----------------------------------------------------------------------------------------------
 
 
-def grad_baseline_dense_torch(sub_adj, sub_feat, pred_label_node, node_idx_new, weights):
+def grad_baseline_dense_torch(sub_adj, sub_feat, pred_label_node, node_idx_new, weights, dtype=np.float32):
     """The reference's gradient baseline, Explainer.explain(model="grad") (explain.py:125-133) with
     ExplainModule.adj_feat_grad (explain.py:717-738), restated: one forward of the frozen model on the UNMASKED
-    sub-adjacency and features, loss = -log softmax(logits[node])[predicted label of the node], one backward w.r.t.
-    the dense adjacency; result sigmoid(|dA| + |dA|^T) * A."""
+    sub-adjacency and features (diagonal included: the reference uses the raw sub_adj), loss = -log softmax(logits[node])
+    [predicted label of the node], one backward w.r.t. the dense adjacency; result sigmoid(|dA| + |dA|^T) * A.
+    dtype=np.float64: the same autograd computation in double precision (inputs and weights cast)."""
     import torch
-    A = torch.tensor(np.asarray(sub_adj, np.float32)[None], dtype=torch.float, requires_grad=True)
-    x = torch.tensor(np.asarray(sub_feat, np.float32)[None], dtype=torch.float, requires_grad=True)
+    tdt = torch.float64 if dtype == np.float64 else torch.float
+    A = torch.tensor(np.asarray(sub_adj, dtype)[None], dtype=tdt, requires_grad=True)
+    x = torch.tensor(np.asarray(sub_feat, dtype)[None], dtype=tdt, requires_grad=True)
     W = weights_to_torch(weights)
+    if tdt == torch.float64:
+        W = dict(conv_w=[w.detach().double() for w in W["conv_w"]],
+                 conv_b=[None if b is None else b.detach().double() for b in W["conv_b"]],
+                 pred_w=W["pred_w"].detach().double(), pred_b=W["pred_b"].detach().double())
     ypred = _gcn_forward_torch(x, A, W, False)
     logit = torch.softmax(ypred[0, node_idx_new, :], dim=0)[int(pred_label_node)]
     loss = -torch.log(logit)
     loss.backward()
     g = torch.abs(A.grad)[0]
     m = torch.sigmoid(g + g.t())
-    return m.detach().numpy() * np.asarray(sub_adj, np.float32)
+    return m.detach().numpy() * np.asarray(sub_adj, dtype)
+
+
+def grad_closed_form(sub_adj, sub_feat, pred_label_node, node_idx_new, weights, dtype=np.float64, return_grad=False):
+    """Hand-derived form of grad_baseline_dense_torch, numpy, any number of layers (no --bn).  The forward runs on sub_adj AS
+    GIVEN -- the reference's raw sub-adjacency, so a self loop (diagonal entry) takes part in the forward and the backward and
+    gets its own result entry sigmoid(2 |dL/dA_ii|).  dL/dA = sum_l dZ_l H_{l-1}^T with dZ_l the gradient at A H_{l-1}.
+    Returns the (n, n) result sigmoid(|dA| + |dA|^T) * A; return_grad=True also returns dA."""
+    f = dtype
+    A = np.asarray(sub_adj, dtype=f)
+    X = np.asarray(sub_feat, dtype=f)
+    n = A.shape[0]
+    Ws, bs = [], []
+    l = 1
+    while ("W%d" % l) in weights:
+        Ws.append(np.asarray(weights["W%d" % l], dtype=f))
+        b = weights.get("b%d" % l)
+        bs.append(np.zeros(Ws[-1].shape[1], f) if b is None else np.asarray(b, dtype=f))
+        l += 1
+    L = len(Ws)
+    dims = [w.shape[1] for w in Ws]
+    offs = np.concatenate([[0], np.cumsum(dims)])
+    Wp = np.asarray(weights["Wp"], dtype=f)
+    bp = np.asarray(weights["bp"], dtype=f)
+    r = int(node_idx_new)
+    H, Yh, q = [X], [], []
+    for l in range(L):
+        Y = (A @ H[-1]) @ Ws[l] + bs[l]                                             # models.py:70-76
+        ql = np.maximum(np.sqrt((Y * Y).sum(1, keepdims=True)), f(1e-12))           # F.normalize eps
+        Yh.append(Y / ql); q.append(ql)
+        H.append(np.maximum(Yh[-1], 0) if l < L - 1 else Yh[-1])
+    emb = np.concatenate([H[l + 1][r] for l in range(L)])
+    logits = Wp @ emb + bp
+    p = np.exp(logits - logits.max()); p = p / p.sum()
+    g = p.copy(); g[int(pred_label_node)] -= 1                                      # d(-log p[pred_label])/dlogits
+    dEmb = Wp.T @ g
+    dA = np.zeros((n, n), f)
+    dH = np.zeros((n, dims[L - 1]), f)
+    for l in range(L - 1, -1, -1):
+        dYh = dH.copy()
+        dYh[r] += dEmb[offs[l]:offs[l + 1]]
+        if l < L - 1:
+            dYh = dYh * (Yh[l] > 0)
+        dY = (dYh - Yh[l] * (Yh[l] * dYh).sum(1, keepdims=True)) / q[l]             # backward of x / max(|x|, eps)
+        dZ = dY @ Ws[l].T
+        dA += dZ @ H[l].T
+        dH = A.T @ dZ
+    G = np.abs(dA)
+    out = _sigmoid(G + G.T) * A
+    return (out, dA) if return_grad else out
 
 
 def _sigmoid(x):

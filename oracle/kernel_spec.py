@@ -235,3 +235,62 @@ def explain_pruned_edges_sparse(rowptr, col, X, gt_label, pred_label, r, weights
             v_ *= f(beta2); v_ += f(1 - beta2) * G_ * G_
             P_ -= step * m_ / (np.sqrt(v_) / b2s + f(eps))
     return (a, F) if return_F else a
+
+
+def grad_edges_sparse(rowptr, col, X, pred_label_node, r, weights, loops=None, dtype=np.float64, chunk=1 << 18):
+    """The gradient baseline (explain.py:125-133,717-738; oracle.grad_closed_form) for subgraphs too large for a dense form:
+    scipy.sparse forward / backward on the full sub-adjacency, dL/dA evaluated only at the CSR slots.  rowptr/col: the local CSR
+    without the diagonal; loops: optional bool (n,) -- the members with a self loop, whose diagonal entry joins the forward and the
+    backward as in the reference's raw sub_adj.  Any number of layers (no --bn).  Returns (slot values, diagonal values) with the
+    diagonal values sigmoid(2 |dL/dA_ii|) where loops is set and 0 elsewhere; slot values sigmoid(|dL/dA_ij| + |dL/dA_ji|)."""
+    import scipy.sparse as sp
+    f = dtype
+    n = len(rowptr) - 1
+    X = np.asarray(X, f)
+    Ws, bs = [], []
+    l = 1
+    while ("W%d" % l) in weights:
+        Ws.append(np.asarray(weights["W%d" % l], f))
+        b = weights.get("b%d" % l)
+        bs.append(np.zeros(Ws[-1].shape[1], f) if b is None else np.asarray(b, f))
+        l += 1
+    L = len(Ws)
+    dims = [w.shape[1] for w in Ws]
+    offs = np.concatenate([[0], np.cumsum(dims)])
+    Wp = np.asarray(weights["Wp"], f); bp = np.asarray(weights["bp"], f)
+    rowptr = np.asarray(rowptr, np.int64); ej = np.asarray(col, np.int64)
+    ei = np.repeat(np.arange(n, dtype=np.int64), np.diff(rowptr))
+    E = len(ej)
+    order = np.lexsort((ei, ej))
+    rev = np.empty(E, np.int64); rev[order] = np.arange(E)
+    assert np.array_equal(ei[rev], ej) and np.array_equal(ej[rev], ei), "sub-adjacency is not symmetric"
+    assert not (ei == ej).any(), "pass self loops through `loops`"
+    dvec = np.zeros(n, f) if loops is None else np.asarray(loops, bool).astype(f)
+    A = sp.csr_matrix((np.ones(E, f), ej, rowptr), shape=(n, n)) + sp.diags(dvec)
+    H, Yh, q = [X], [], []
+    for l in range(L):
+        Y = (A @ H[-1]) @ Ws[l] + bs[l]
+        ql = np.maximum(np.sqrt((Y * Y).sum(1, keepdims=True)), f(1e-12))
+        Yh.append(Y / ql); q.append(ql)
+        H.append(np.maximum(Yh[-1], 0) if l < L - 1 else Yh[-1])
+    emb = np.concatenate([H[l + 1][r] for l in range(L)])
+    logits = Wp @ emb + bp
+    p = np.exp(logits - logits.max()); p /= p.sum()
+    g = p.copy(); g[int(pred_label_node)] -= 1
+    dEmb = Wp.T @ g
+    gA = np.zeros(E, f)
+    gD = np.zeros(n, f)
+    dH = np.zeros((n, dims[L - 1]), f)
+    for l in range(L - 1, -1, -1):
+        dYh = dH.copy()
+        dYh[r] += dEmb[offs[l]:offs[l + 1]]
+        if l < L - 1:
+            dYh = dYh * (Yh[l] > 0)
+        dY = (dYh - Yh[l] * (Yh[l] * dYh).sum(1, keepdims=True)) / q[l]
+        dZ = dY @ Ws[l].T
+        for s0 in range(0, E, chunk):                          # SDDMM: dL/dA_ij = <dZ_i, H_j> at the slots
+            gA[s0:s0 + chunk] += np.einsum("ij,ij->i", dZ[ei[s0:s0 + chunk]], H[l][ej[s0:s0 + chunk]])
+        gD += np.einsum("ij,ij->i", dZ, H[l])
+        dH = A.T @ dZ
+    G = np.abs(gA)
+    return _sigmoid(G + G[rev]), np.where(dvec > 0, _sigmoid(2 * np.abs(gD)), 0.0)
