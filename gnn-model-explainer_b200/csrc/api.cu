@@ -224,7 +224,7 @@ int launch_var_batch(gx_handle* h, const char* who, int graph_mode, const GxHpar
   return GX_OK;
 }
 
-// Model variant (num_gc_layers 2 / 4, --bn, widths 33..128, attention, inputs wider than 128): explain_var.cu, true widths (a zero-padded column would enter
+// Model variant (num_gc_layers 2 / 4 .. 7, --bn, widths 33..128, attention, inputs wider than 128): explain_var.cu, true widths (a zero-padded column would enter
 // the bn statistics).  att_w != nullptr: an attention model, each layer's (in, in) attention weights right after its conv weights
 // (gx_att_weight).  The widths were checked by the caller.
 static int set_variant_model(gx_handle* h, const char* who, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
@@ -269,7 +269,8 @@ static int set_variant_model(gx_handle* h, const char* who, const gx_model_dims*
 // The dimension checks of gx_set_model / gx_set_model_att
 static int check_model_dims(const char* who, const gx_model_dims* dims) {
   if (dims->num_layers < 2 || dims->num_layers > GX_MAX_LAYERS) {
-    gx_set_error("%s: num_layers=%d outside [2,%d]", who, dims->num_layers, GX_MAX_LAYERS);
+    gx_set_error("%s: num_layers=%d outside [2,%d] (the k-hop planner's limit: n_hops = num_layers <= %d)", who, dims->num_layers, GX_MAX_LAYERS,
+                 GX_MAX_LEVELS - 1);
     return GX_ERR_UNSUPPORTED;
   }
   if (dims->hidden_dim < 1 || dims->embed_dim < 1 || dims->hidden_dim > 128 || dims->embed_dim > 128) {
@@ -430,14 +431,14 @@ int gx_model_forward(gx_handle* h, gx_memspace space, float* pred) {
   if (!h || !pred) { gx_set_error("gx_model_forward: NULL argument"); return GX_ERR_INVALID; }
   if (!h->has_graph || !h->has_model) { gx_set_error("gx_model_forward: call gx_set_model and gx_set_graph_csr first"); return GX_ERR_INVALID; }
   if (h->g.d != h->m.d) { gx_set_error("gx_model_forward: graph feat_dim %d != model input_dim %d", h->g.d, h->m.d); return GX_ERR_INVALID; }
-  if (h->m.hid > 32 || h->m.emb > 32) { gx_set_error("gx_model_forward: widths > 32 are not built (pass pred to the Explainer)"); return GX_ERR_UNSUPPORTED; }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
   const size_t np_ = (size_t)h->g.N * h->m.C;
+  const size_t nh = (size_t)h->m.L * h->g.N * gx_var_row_stride(h->m.hid, h->m.emb);   // every layer's rows, 32 / 64 / 128 floats each
   const size_t npw = h->m.att ? (size_t)h->g.N * gx_round_up(std::max(h->m.d, h->m.hid), 4) : 0;   // attention models: P
-  GX_CUDA_CHECK(h->d_fwd.reserve(((size_t)h->m.L * h->g.N * 32 + np_ + npw) * 4));
+  GX_CUDA_CHECK(h->d_fwd.reserve((nh + np_ + npw) * 4));
   float* H = h->d_fwd.as<float>();
-  float* pd = space == GX_DEVICE ? pred : H + (size_t)h->m.L * h->g.N * 32;
-  float* P = h->m.att ? H + (size_t)h->m.L * h->g.N * 32 + np_ : nullptr;
+  float* pd = space == GX_DEVICE ? pred : H + nh;
+  float* P = h->m.att ? H + nh + np_ : nullptr;
   GX_CUDA_CHECK(gx_launch_model_forward(h->g, h->m, H, pd, nullptr, P, h->stream));
   h->launches += h->m.L * (h->m.att ? 2 : 1) + 1;
   if (space != GX_DEVICE) {

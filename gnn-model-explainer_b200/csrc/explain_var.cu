@@ -1,6 +1,6 @@
 // explain_var.cu -- K2v: the mask-optimisation kernel for the model and optimiser VARIANTS of the reference (SURVEY 8 row f3), node
 // mode and graph-classification mode:
-//   num_gc_layers = 2 / 3 / 4 (explainer_main.py:57-66, explain.py:64: n_hops = num_gc_layers; models.py:193-220,230-267) and
+//   num_gc_layers = 2 .. 7 (explainer_main.py:57-66, explain.py:64: n_hops = num_gc_layers; models.py:193-220,230-267) and
 //   --bn (models.py:222-228: a FRESH BatchNorm1d(n) in train mode on the (1, n, h) activations = per-node standardisation over
 //   the feature axis, eps 1e-5, biased variance, applied after the ReLU of every hidden layer; the readout concatenates the
 //   standardised activations, models.py:241-260), hidden / output widths up to 128 (the tuned kernels stop at 32), d <= 128, and

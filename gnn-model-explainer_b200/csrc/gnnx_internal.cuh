@@ -8,7 +8,7 @@
 
 #define GX_MAX_LEVELS 8  // n_hops <= 7
 #define GX_NONE16 0xFFFFu
-#define GX_MAX_LAYERS 4  // num_gc_layers of a model variant (explain_var.cu); the tuned kernels build the reference default 3
+#define GX_MAX_LAYERS 7  // num_gc_layers of a model variant (explain_var.cu): n_hops = num_gc_layers < GX_MAX_LEVELS; the tuned kernels build the reference default 3
 #define GX_MAX_GANG 160   // CTAs that may share one task in explain_gang.cu (<= number of SMs)
 #define GX_GRID_CAP (132 * 8)  // CTAs of a grid-stride launch: 8 per SM of an H100 (132 SMs)
 #define GX_WP_SMEM_MAX 2048  // floats: pred_model (C x (2h+e) + C) is kept in shared memory up to this size

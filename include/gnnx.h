@@ -47,7 +47,7 @@ typedef struct gx_model_dims {
   int32_t hidden_dim;  /* output width of conv_first / conv_block[*]    */
   int32_t embed_dim;   /* output width of conv_last                     */
   int32_t num_classes; /* label_dim                                     */
-  int32_t num_layers;  /* num_gc_layers: 2, 3 (reference default) or 4    */
+  int32_t num_layers;  /* num_gc_layers: 2 .. 7 (reference default 3)     */
   int32_t flags;       /* GX_MODEL_* bits                               */
 } gx_model_dims;
 #define GX_MODEL_BN 1u /* args.bn (models.py:222-228): per-node standardisation after every hidden ReLU.  num_layers != 3, bn, att or
@@ -227,7 +227,7 @@ int gx_set_graph_batch_csr(gx_handle* h, int32_t num_graphs, int32_t max_nodes, 
 /* Plans the graphs to explain; edge_off[count+1] (may be NULL) receives the packed slot offsets: the slots of
  * graph t are the entries of its adjacency in row-major order (its slice of the CSR).  Any model gx_set_model accepts:
  * the default model needs every graph to fit the tuned kernel's shared memory (GX_ERR_UNSUPPORTED otherwise); a model
- * variant (2 / 4 layers, --bn, widths 33..128) keeps each graph in device memory, bounded by max_nodes <= 4096 only. */
+ * variant (2 or 4 .. 7 layers, --bn, widths 33..128) keeps each graph in device memory, bounded by max_nodes <= 4096 only. */
 int gx_plan_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int64_t* edge_off, int64_t* total_edges);
 /* Explainer.explain(node_idx=0, graph_idx=g, graph_mode=True) for every planned graph (model =
  * GcnEncoderGraph: per-layer max-pool readout, models.py:269-316; lap_loss = 0, explain.py:787-788).

@@ -3,7 +3,7 @@
     compute-sanitizer --tool racecheck python tools/sanitize_run.py
 k-hop extraction + shared-memory kernel on a mix of task sizes (syn1: hub node 0 and tiny tasks), the streaming kernel (forced),
 the gradient baseline, graph mode, densify, the off-edge regulariser sums of graph mode, neighbourhood rows, the unconstrained (dense) kernel, attention models, inputs wider than 128
-features (explain_var.cu's wide path).  A few epochs each."""
+features (explain_var.cu's wide path), models with 5 to 7 layers.  A few epochs each."""
 import os
 import sys
 
@@ -86,6 +86,40 @@ def main():
         eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS, opt=1, init=_abi.GX_INIT_PHILOX, seed=3), None, out)
         print("var ok graph sgd", float(out.sum()))
         eng.close()
+        # deep models (num_gc_layers 5 .. 7): L = 7 with --bn and widths 128 (conv weights and pred_model through L2), L = 5 attention,
+        # node mode (hub and small tasks, 7 hops) and graph mode, the model forward with 128-float rows, the unconstrained kernel at L = 7
+        for L, hid, bn, att in ((7, 128, True, False), (5, 20, False, True), (6, 64, False, False)):
+            dims = [d0] + [hid] * L
+            w = {}
+            for l in range(1, L + 1):
+                w["W%d" % l] = sc(dims[l - 1], dims[l]); w["b%d" % l] = sc(dims[l])
+                if att:
+                    w["Wa%d" % l] = sc(dims[l - 1], dims[l - 1])
+            w["Wp"], w["bp"] = sc(3, hid * L), sc(3)
+            attw = [w["Wa%d" % l] for l in range(1, L + 1)] if att else None
+            eng = gnnx.Engine(0)
+            eng.set_model(w, num_layers=L, bn=bn, att=attw)
+            eng.set_graph_csr(rowptr, col, g["feat"].astype(np.float32), g["label"].astype(np.int32), np.zeros(N, np.int32))
+            plan = eng.plan_nodes([0, 17], L)
+            out = np.zeros(plan.total_edges, np.float32)
+            eng.explain_nodes_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=2), None, out)
+            pred = eng.model_forward()
+            if not att:
+                eng.explain_nodes_unconstrained(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=4), None, out)
+            print("var ok deep node", L, hid, bn, att, float(out.sum()), float(pred.sum()))
+            eng.close()
+            wg = dict(w)
+            wg["W1"] = sc(gg["feat"].shape[2], hid)
+            if att:
+                wg["Wa1"] = sc(gg["feat"].shape[2], gg["feat"].shape[2]); attw[0] = wg["Wa1"]
+            eng = gnnx.Engine(0)
+            eng.set_model(wg, num_layers=L, bn=bn, att=attw)
+            eng.set_graph_batch(gg["adj"], gg["feat"], gg["label"] % 3)
+            eoff = eng.plan_graphs([0, 3, 5])
+            out = np.zeros(int(eoff[-1]), np.float32)
+            eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=3), None, out)
+            print("var ok deep graph", L, hid, bn, att, float(out.sum()))
+            eng.close()
     if "cluster" in which:
         eng = util.make_engine(fx)
         eng.debug_cluster(4, 1)
