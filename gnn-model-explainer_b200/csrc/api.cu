@@ -224,7 +224,7 @@ int launch_var_batch(gx_handle* h, const char* who, int graph_mode, const GxHpar
   return GX_OK;
 }
 
-// Model variant (num_gc_layers 2 / 4 .. 7, --bn, widths 33..128, attention, inputs wider than 128): explain_var.cu, true widths (a zero-padded column would enter
+// Model variant (num_gc_layers 2 / 4 .. 7, --bn, widths 33..256, attention, inputs wider than 128): explain_var.cu, true widths (a zero-padded column would enter
 // the bn statistics).  att_w != nullptr: an attention model, each layer's (in, in) attention weights right after its conv weights
 // (gx_att_weight).  The widths were checked by the caller.
 static int set_variant_model(gx_handle* h, const char* who, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
@@ -273,8 +273,9 @@ static int check_model_dims(const char* who, const gx_model_dims* dims) {
                  GX_MAX_LEVELS - 1);
     return GX_ERR_UNSUPPORTED;
   }
-  if (dims->hidden_dim < 1 || dims->embed_dim < 1 || dims->hidden_dim > 128 || dims->embed_dim > 128) {
-    gx_set_error("%s: hidden_dim=%d output_dim=%d; this build supports widths up to 128 (tuned kernels up to 32, the variant kernel beyond)", who, dims->hidden_dim, dims->embed_dim);
+  if (dims->hidden_dim < 1 || dims->embed_dim < 1 || dims->hidden_dim > GX_MAX_WIDTH || dims->embed_dim > GX_MAX_WIDTH) {
+    gx_set_error("%s: hidden_dim=%d output_dim=%d; this build supports widths up to GX_MAX_WIDTH = %d (tuned kernels up to 32, the variant kernel beyond)",
+                 who, dims->hidden_dim, dims->embed_dim, GX_MAX_WIDTH);
     return GX_ERR_UNSUPPORTED;
   }
   if (dims->input_dim < 1 || dims->input_dim > GX_VAR_WIDE_MAX) {
@@ -433,7 +434,7 @@ int gx_model_forward(gx_handle* h, gx_memspace space, float* pred) {
   if (h->g.d != h->m.d) { gx_set_error("gx_model_forward: graph feat_dim %d != model input_dim %d", h->g.d, h->m.d); return GX_ERR_INVALID; }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
   const size_t np_ = (size_t)h->g.N * h->m.C;
-  const size_t nh = (size_t)h->m.L * h->g.N * gx_var_row_stride(h->m.hid, h->m.emb);   // every layer's rows, 32 / 64 / 128 floats each
+  const size_t nh = (size_t)h->m.L * h->g.N * gx_var_row_stride(h->m.hid, h->m.emb);   // every layer's rows, 32 / 64 / 128 / 256 floats each
   const size_t npw = h->m.att ? (size_t)h->g.N * gx_round_up(std::max(h->m.d, h->m.hid), 4) : 0;   // attention models: P
   GX_CUDA_CHECK(h->d_fwd.reserve((nh + np_ + npw) * 4));
   float* H = h->d_fwd.as<float>();
@@ -540,6 +541,11 @@ int gx_set_model_att(gx_handle* h, const gx_model_dims* dims, const float* const
   if (rc != GX_OK) return rc;
   if (dims->input_dim >= GX_VAR_WIDE_MIN) {
     gx_set_error("gx_set_model_att: input_dim=%d; attention models are built for inputs up to 128 wide (layer 1's attention matrix is input_dim x input_dim)", dims->input_dim);
+    return GX_ERR_UNSUPPORTED;
+  }
+  if (dims->hidden_dim > 128 || dims->embed_dim > 128) {
+    gx_set_error("gx_set_model_att: hidden_dim=%d output_dim=%d; attention models are built for widths up to 128 (widths above 128 run the "
+                 "variant kernel's row-block path, which has no attention layers)", dims->hidden_dim, dims->embed_dim);
     return GX_ERR_UNSUPPORTED;
   }
   GX_CUDA_CHECK(cudaSetDevice(h->device));

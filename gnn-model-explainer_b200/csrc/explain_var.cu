@@ -3,7 +3,7 @@
 //   num_gc_layers = 2 .. 7 (explainer_main.py:57-66, explain.py:64: n_hops = num_gc_layers; models.py:193-220,230-267) and
 //   --bn (models.py:222-228: a FRESH BatchNorm1d(n) in train mode on the (1, n, h) activations = per-node standardisation over
 //   the feature axis, eps 1e-5, biased variance, applied after the ReLU of every hidden layer; the readout concatenates the
-//   standardised activations, models.py:241-260), hidden / output widths up to 128 (the tuned kernels stop at 32), d <= 128, and
+//   standardised activations, models.py:241-260), hidden / output widths up to 256 (the tuned kernels stop at 32), d <= 128, and
 //   the optimisers of utils/train_utils.py:7-23 (Adam, SGD momentum 0.95, RMSprop, Adagrad; step / cos schedulers).
 // Node mode computes exactly what oracle/kernel_spec.py specifies (parameters on the directed edges, layer l only on the rows within
 // L - l hops of the explained node, inner / outer pair split) and reads out row 0 (the explained node in level order).
@@ -32,6 +32,13 @@
 //   B0  G = X^T dP (3xTF32), dL/dsF_f = sum_c W1_fc G_fc;
 //   P   layer 1's pair term <dY1_i, P_j> + <dY1_j, P_i> replaces the d-wide dots.
 // The feature-mask state and the products live in the task slab and W1 is read through L2, so shared memory does not grow with d.
+// Hidden / output widths of 129 .. 256 (kBlk, KW = 8, no attention; DESIGN section 15) take each layer's product over the row block
+// instead of row by row, so that a 256 x 256 weight read through L2 is not re-read per row:
+//   Fl  gather Z = A_m H_{l-1} (layer 1: U = A_m X) of the layer's rows, then Y = b + Z W_l (rows_product, FP32) into Yh(l), then the
+//       row epilogue (normalise, ReLU, bn) in place; Z lives in dZ(l), which the backward overwrites;
+//   Bl  the row backward writes dY over the row's Yh(l), then dZ_l = dY W_l^T over the block (layer 1: into dZ1, then dL/dsF's partials
+//       and dZ1 (.) sF row by row, as var_first_layer_dz).
+// The slab and shared-memory carve-ups are the narrow ones with 256-float rows.
 #include "explain_var_common.cuh"
 #include "mma_tf32.cuh"
 
@@ -195,10 +202,36 @@ __device__ __forceinline__ void wide_mma(int M, int N, int K, FA a, FB b, float*
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------ hidden widths 129 .. 256
+// C = bias + A B (M x N, row stride ldc; bias == nullptr: 0) in FP32 on the CUDA cores: a warp takes 8 rows x 32 columns at a time
+// (lane = column, one accumulator per row), k in ascending order.  Each output is the chain fmaf(a(r, k), b(k, c), .) from the bias that
+// var_dense / var_hidden_dz / var_first_layer_dz compute for a single row, so the row-block path does the narrow path's arithmetic, and a
+// B row is read once per 8 rows.  a(r, k) and b(k, c) return the operands and 0 outside the matrices.
+template <typename FA, typename FB>
+__device__ __forceinline__ void rows_product(int M, int N, int K, FA a, FB b, const float* bias, float* C, int ldc, int warp, int nwarps, int lane) {
+  constexpr int RB = 8;
+  const int tn = (N + 31) / 32, tiles = (M + RB - 1) / RB * tn;
+  for (int tile = warp; tile < tiles; tile += nwarps) {
+    const int r0 = tile / tn * RB, c = tile % tn * 32 + lane;
+    float acc[RB];
+#pragma unroll
+    for (int r = 0; r < RB; ++r) acc[r] = bias != nullptr && c < N ? bias[c] : 0.f;
+    for (int k = 0; k < K; ++k) {
+      const float bk = b(k, c);
+#pragma unroll
+      for (int r = 0; r < RB; ++r) acc[r] = fmaf(a(r0 + r, k), bk, acc[r]);
+    }
+#pragma unroll
+    for (int r = 0; r < RB; ++r)
+      if (r0 + r < M && c < N) C[(int64_t)(r0 + r) * ldc + c] = acc[r];
+  }
+}
+
 // The minimum-blocks bound 0 is the compiler's default: node mode is capped at 128 registers (some instantiations spill); graph mode
 // lets the small default-width model fit two CTAs per SM.
-template <bool kGraph, bool kBn, int KW, bool kAtt, bool kWide>
+template <bool kGraph, bool kBn, int KW, bool kAtt, bool kWide, bool kBlk = false>
 __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1) : 0) explain_var_kernel(const VarArgs A) {
+  static_assert(!kBlk || (KW == 8 && !kAtt), "the row-block path is built for widths 129 .. 256 without attention");
   extern __shared__ __align__(16) float sm[];
   __shared__ int s_task;
   constexpr int NT = kVarThreads, nwarps = NT / 32;
@@ -356,11 +389,36 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
               continue;
             }
           }
+          if constexpr (kBlk) {   // the aggregate only (layer 1: U; above: Z into dZ(l), free until the backward)
+            if (l == 1) var_gather_feat(r0, r1, icol, a, feat, lo2gid, d, sF, U + (int64_t)i * dp, zs, lane);
+            else var_gather_hidden<KW>(r0, r1, icol, a, Hh(l - 1), win, dZ(l) + (int64_t)i * VW, lane);
+            continue;
+          }
           if (l == 1) var_gather_feat(r0, r1, icol, ag, feat, lo2gid, d, sF, U + (int64_t)i * dp, zs, lane);
           else var_gather_hidden<KW>(r0, r1, icol, ag, Hh(l - 1), win, zs, lane);
           var_row_forward<kBn, KW>(zs, win, Ws, wout, bsm, l, L, i, Yh, Hh, VW, qn, istd, lane);
         }
         __syncthreads();
+        if constexpr (kBlk) {
+          if (!kWide || l > 1) {   // Y = b + Z W over the layer's rows into Yh(l), then the row epilogue in place
+            const int nr = rows(l);
+            float* const Zl = l == 1 ? U : dZ(l);
+            const int ldz = l == 1 ? dp : VW;
+            rows_product(nr, wout, win, [&](int r, int k) { return r < nr ? (l == 1 ? Zl[(int64_t)r * ldz + k] * sF[k] : Zl[(int64_t)r * ldz + k]) : 0.f; },
+                         [&](int k, int c) { return c < wout ? Ws[k * wout + c] : 0.f; }, bsm, Yh(l), VW, warp, nwarps, lane);
+            __syncthreads();
+            for (int i = warp; i < nr; i += nwarps) {
+              float y[KW];
+#pragma unroll
+              for (int k = 0; k < KW; ++k) {
+                const int c = lane + 32 * k;
+                y[k] = c < wout ? Yh(l)[(int64_t)i * VW + c] : 0.f;
+              }
+              var_row_epilogue<kBn, KW>(y, wout, l, L, i, Yh, Hh, VW, qn, istd, lane);
+            }
+            __syncthreads();
+          }
+        }
       }
       // ---------------------------------------------------------------- S: readout, softmax, dEmb   (models.py:305-314, explain.py:711)
       if constexpr (kGraph) {   // max-pool of every layer, the edge-less rows' constant first
@@ -400,6 +458,11 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
             if (c < wout && (kGraph ? arg[koff + c] == i : i == 0)) g[k] += dEmb[koff + c];
             yh[k] = Yh(l)[(int64_t)i * VW + c];
           }
+          if constexpr (kBlk) {   // dY straight into the slab: over the row's Yh (read above, not read again; the product runs over the
+                                  // row block below), or into dY1 on the wide input path's layer 1
+            var_row_backward<kBn, KW>(g, yh, l, L, i, Hh, VW, qn, istd, wout, (kWide && l == 1 ? dY1 : Yh(l)) + (int64_t)i * VW, lane);
+            continue;
+          }
           var_row_backward<kBn, KW>(g, yh, l, L, i, Hh, VW, qn, istd, wout, zs, lane);
           if constexpr (kWide) {
             if (l == 1) {   // B1: keep dY1
@@ -415,6 +478,25 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
           __syncwarp();
         }
         __syncthreads();
+        if constexpr (kBlk) {
+          if (!kWide || l > 1) {   // dZ = dY W^T over the layer's rows (layer 1: into dZ1, then dL/dsF's partials and the mask)
+            const int nr = rows(l);
+            const float* const dYl = Yh(l);
+            rows_product(nr, win, wout, [&](int r, int c) { return r < nr ? dYl[(int64_t)r * VW + c] : 0.f; },
+                         [&](int c, int f) { return f < win ? Ws[f * wout + c] : 0.f; }, nullptr, l == 1 ? dZ1 : dZ(l), l == 1 ? dp : VW,
+                         warp, nwarps, lane);
+            __syncthreads();
+            if (l == 1) {   // as var_first_layer_dz: each warp's rows in ascending order into its own partials
+              for (int i = warp; i < nr; i += nwarps)
+                for (int f = lane; f < d; f += 32) {
+                  const float t = dZ1[(int64_t)i * dp + f];
+                  gFp[warp * dp + f] = fmaf(t, U[(int64_t)i * dp + f], gFp[warp * dp + f]);
+                  dZ1[(int64_t)i * dp + f] = t * sF[f];
+                }
+              __syncthreads();
+            }
+          }
+        }
         if constexpr (kWide) {
           if (l == 1) {
             // B1: dP_j = sum_i a_ij dY1_i over j's leading columns that are layer-1 rows (A_m symmetric), every row j of the task
@@ -554,6 +636,16 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
 // calls f(kernel) with the instantiation for the mode and the model
 template <typename F>
 cudaError_t with_var_kernel(int graph_mode, const GxModelDev& m, F&& f) {
+  if (var_row_kw(m.hid, m.emb) == 8) {   // widths 129 .. 256: the row-block path (attention models are refused at these widths)
+    if (m.att) return cudaErrorInvalidValue;
+    const bool wide = m.d >= GX_VAR_WIDE_MIN;
+    auto blk = [&](auto bn) {
+      constexpr bool b = decltype(bn)::value;
+      if (graph_mode) return wide ? f(explain_var_kernel<true, b, 8, false, true, true>) : f(explain_var_kernel<true, b, 8, false, false, true>);
+      return wide ? f(explain_var_kernel<false, b, 8, false, true, true>) : f(explain_var_kernel<false, b, 8, false, false, true>);
+    };
+    return m.bn ? blk(std::true_type()) : blk(std::false_type());
+  }
   return var_dispatch(m, [&](auto bn, auto kw) {
     constexpr bool b = decltype(bn)::value;
     constexpr int w = decltype(kw)::value;
@@ -572,7 +664,7 @@ int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C, int
                                          : var_smem(d, L, hid, emb, C, kVarThreads / 32, att).total;
   return (words + pool) * 4;
 }
-int gx_var_row_stride(int hid, int emb) { return 32 * var_kw(hid, emb); }
+int gx_var_row_stride(int hid, int emb) { return 32 * var_row_kw(hid, emb); }
 
 int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m) {
   const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C, m.att);

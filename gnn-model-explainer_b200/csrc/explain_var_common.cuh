@@ -1,7 +1,8 @@
 // explain_var_common.cuh -- the per-row and per-parameter steps and the launch code shared by the model-variant kernel
 // (explain_var.cu, node and graph mode) and the unconstrained kernel (explain_dense.cu).  Both are written for clarity, not speed:
-// one persistent CTA per task, one warp per row with lane = feature, KW chunks of 32 lanes for widths up to 128 (chunk k holds
-// features 32k + lane), the TRUE widths (no zero padding: a padded column would enter the bn statistics), state in a per-CTA global slab.
+// one persistent CTA per task, one warp per row with lane = feature, KW chunks of 32 lanes for widths up to 128, or 256 on the
+// variant kernel's row-block path (chunk k holds features 32k + lane), the TRUE widths (no zero padding: a padded column would enter
+// the bn statistics), state in a per-CTA global slab.
 #pragma once
 #include <type_traits>
 
@@ -14,6 +15,9 @@ constexpr int kVarWeightWords = 36 * 1024;   // conv weights are staged in share
 
 // KW = 32-lane chunks of a hidden-width row: 1 for widths <= 32, 2 <= 64, 4 <= 128
 __host__ __device__ inline int var_kw(int hid, int emb) { const int w = hid > emb ? hid : emb; return w <= 32 ? 1 : (w <= 64 ? 2 : 4); }
+// the same with 8 for widths 129 .. 256 (explain_var.cu's row-block path: its per-warp scratch rows stay var_kw wide, the dY rows are
+// written to the slab in place)
+inline int var_row_kw(int hid, int emb) { return (hid > emb ? hid : emb) > 128 ? 8 : var_kw(hid, emb); }
 
 // Shared-memory carve-up (words) of the model-variant kernels: conv weights (when they fit) and biases, pred_model, the feature-mask
 // state, per-warp scratch rows and partial dL/dsF, the readout vectors.  Attention models (att != 0) also stage the (in, in)
@@ -408,12 +412,14 @@ __device__ __forceinline__ void var_max_pool(int L, int hid, int PD, int n, Hl H
 }
 
 // ------------------------------------------------------------------------------------------------------------------------- launch
-// Calls f(std::integral_constant<bool, kBn>, std::integral_constant<int, KW>) with the model's instantiation.
+// Calls f(std::integral_constant<bool, kBn>, std::integral_constant<int, KW>) with the model's instantiation, widths up to 128 (wider
+// rows have no instantiation here: explain_var.cu dispatches its row-block path itself).
 template <typename F>
 cudaError_t var_dispatch(const GxModelDev& m, F&& f) {
   using B = std::integral_constant<bool, true>;
   using N = std::integral_constant<bool, false>;
-  const int kw = var_kw(m.hid, m.emb);
+  const int kw = var_row_kw(m.hid, m.emb);
+  if (kw > 4) return cudaErrorInvalidValue;
   if (m.bn) {
     if (kw == 1) return f(B(), std::integral_constant<int, 1>());
     if (kw == 2) return f(B(), std::integral_constant<int, 2>());

@@ -1,8 +1,8 @@
 // forward.cu -- the GCN forward of the reference model on the WHOLE graph (models.py:58-80 GraphConv.forward, :230-267 gcn_forward,
 // :363-376 GcnEncoderNode.forward): what produces the `pred` the Explainer is constructed with (explainer_main.py:186-193 reads it
 // from the checkpoint; `Explainer(pred=None)` computes it here).  Unmasked adjacency, no feature mask, every model gx_set_model accepts
-// (num_layers 2 .. 7, widths up to 128, --bn).  One launch per layer (a layer reads every row of the previous one), a warp per node with
-// lane = feature (1, 2 or 4 chunks of 32 lanes) -- the same row
+// (num_layers 2 .. 7, widths up to 256, --bn).  One launch per layer (a layer reads every row of the previous one), a warp per node with
+// lane = feature (1, 2, 4 or 8 chunks of 32 lanes) -- the same row
 // arithmetic as explain_var.cu: Y = (sum_{j in N(i)} H_{l-1}[j]) W_l + b_l, row L2-normalise, ReLU (+ per-node standardisation
 // with --bn) on hidden layers; logits = pred_model(concat of the layer outputs).  Attention models (--method att, models.py:62-68) first
 // project P = H_{l-1} Wa_l (att_project_kernel) and weight every edge, self loops included, by s_ij = P_i . P_j.
@@ -179,5 +179,6 @@ cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, fl
   const int kw = gx_var_row_stride(m.hid, m.emb) / 32;
   if (kw == 1) return model_forward<1>(g, m, H, pred, emb_out, P, s);
   if (kw == 2) return model_forward<2>(g, m, H, pred, emb_out, P, s);
-  return model_forward<4>(g, m, H, pred, emb_out, P, s);
+  if (kw == 4) return model_forward<4>(g, m, H, pred, emb_out, P, s);
+  return model_forward<8>(g, m, H, pred, emb_out, P, s);
 }

@@ -23,6 +23,10 @@ static int explain_unconstrained_impl(gx_handle* h, bool graph, const gx_hparams
     gx_set_error("%s: inputs wider than 128 (input_dim=%d) are not built for the unconstrained mask", who, h->m.d);
     return GX_ERR_UNSUPPORTED;
   }
+  if (h->has_model && (h->m.hid > 128 || h->m.emb > 128)) {
+    gx_set_error("%s: hidden / output widths above 128 (hidden_dim=%d output_dim=%d) are not built for the unconstrained mask", who, h->m.hid, h->m.emb);
+    return GX_ERR_UNSUPPORTED;
+  }
   if (hp->init == GX_INIT_STATE) { gx_set_error("%s: GX_INIT_STATE is not built for the unconstrained mask", who); return GX_ERR_UNSUPPORTED; }
   if (hp->init == GX_INIT_M0 && !m0_dense) { gx_set_error("%s: GX_INIT_M0 needs m0_dense", who); return GX_ERR_INVALID; }
   if (trace_pred && !trace) { gx_set_error("%s: trace_pred needs trace", who); return GX_ERR_INVALID; }

@@ -114,7 +114,8 @@ class Explainer:
         # model / optimiser variants run in the variant kernel, which does not log the per-epoch trace print_training replays: the
         # selection of gx_set_model (--bn, num_gc_layers != 3, hidden or output widths above 32, inputs wider than 128, attention)
         # and every optimiser other than Adam
-        self._wide_layers = max(weights["W%d" % l].shape[1] for l in range(1, num_layers + 1)) > 32
+        self._max_width = max(weights["W%d" % l].shape[1] for l in range(1, num_layers + 1))
+        self._wide_layers = self._max_width > 32
         self._no_trace = (bn or num_layers != 3 or self._wide_layers or getattr(args, "opt", "adam") != "adam" or self._att
                           or self._wide)
         adj_np = np.asarray(adj)
@@ -259,6 +260,7 @@ class Explainer:
             raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
         if unconstrained and self._wide:
             raise NotImplementedError("unconstrained=True is not built for inputs wider than 128 features")
+        self._check_unconstrained_width(unconstrained)
         hp, init = self._hparams()
         if unconstrained:
             # explain.py:688-692: the dense mask drives the forward, so every one of the n^2 normals of M0 is a parameter
@@ -285,6 +287,10 @@ class Explainer:
         off = self.engine.offedge_regularisers(hp, np.concatenate([D.reshape(-1) for D in dense])) if dense is not None else None
         self.last_trace = self._print_trace(hp, trace, pred, off, np.diff(plan.node_off).astype(np.float64) ** 2)
         return plan, edge_mask
+
+    def _check_unconstrained_width(self, unconstrained):
+        if unconstrained and self._max_width > 128:
+            raise NotImplementedError("unconstrained=True is not built for hidden / output widths above 128 (this model: %d)" % self._max_width)
 
     def _print_no_trace(self):
         if self._att:
@@ -327,6 +333,7 @@ class Explainer:
             raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
         if unconstrained and self._wide:
             raise NotImplementedError("unconstrained=True is not built for inputs wider than 128 features")
+        self._check_unconstrained_width(unconstrained)
         gids = [int(g) for g in graph_indices]
         edge_off = self.engine.plan_graphs(gids)
         hp, init = self._hparams()

@@ -44,15 +44,18 @@ typedef enum gx_memspace { GX_HOST = 0, GX_DEVICE = 1 } gx_memspace;
  * num_layers, bn=..., args.bias) -- reference models.py:84-97,332-345. */
 typedef struct gx_model_dims {
   int32_t input_dim;   /* d: 1..4096.  d > 128 runs on the model-variant kernel's wide path (any layers / bn / widths; not attention models) */
-  int32_t hidden_dim;  /* output width of conv_first / conv_block[*]    */
-  int32_t embed_dim;   /* output width of conv_last                     */
+  int32_t hidden_dim;  /* output width of conv_first / conv_block[*]: 1 .. GX_MAX_WIDTH */
+  int32_t embed_dim;   /* output width of conv_last: 1 .. GX_MAX_WIDTH  */
   int32_t num_classes; /* label_dim                                     */
   int32_t num_layers;  /* num_gc_layers: 2 .. 7 (reference default 3)     */
   int32_t flags;       /* GX_MODEL_* bits                               */
 } gx_model_dims;
 #define GX_MODEL_BN 1u /* args.bn (models.py:222-228): per-node standardisation after every hidden ReLU.  num_layers != 3, bn, att or
-                        * a hidden / output width of 33..128 or an input width above 128 select the model-variant kernels (node mode
-                        * and graph mode, mask optimisation only: no trace / optimiser state / grad / unconstrained masks for d > 128) */
+                        * a hidden / output width of 33..256 or an input width above 128 select the model-variant kernels (node mode
+                        * and graph mode, mask optimisation only: no trace / optimiser state / grad; no unconstrained masks for d > 128
+                        * or for hidden / output widths above 128) */
+#define GX_MAX_WIDTH 256 /* the widest hidden / output width gx_set_model accepts (129 .. 256: the variant kernel's row-block path;
+                          * attention models stop at 128) */
 #define GX_MODEL_ATT 2u /* args.method == "att" (models.py:62-68): every layer scales the adjacency by s_ij = P_i . P_j, P = H Wa.
                          * Set by gx_set_model_att only (gx_set_model refuses it: the attention weights arrive with that call). */
 
@@ -146,7 +149,8 @@ int gx_set_model(gx_handle* h, const gx_model_dims* dims, const float* const* co
 /* Attention model (train.py / explainer_main.py --method att): gx_set_model's arguments plus att_w, num_layers pointers to the
  * row-major (in, in) conv_first.att_weight / conv_block.i.att_weight / conv_last.att_weight.  GX_MODEL_ATT in dims->flags is
  * implied.  Runs on the model-variant kernel (mask optimisation only: no trace, optimiser state, GX_INIT_STATE or grad;
- * no unconstrained mask).  GX_ERR_UNSUPPORTED when the model does not fit the kernel's shared memory. */
+ * no unconstrained mask).  GX_ERR_UNSUPPORTED when the model does not fit the kernel's shared memory or a hidden / output width
+ * is above 128. */
 int gx_set_model_att(gx_handle* h, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
                      const float* const* att_w, const float* pred_w, const float* pred_b);
 
@@ -227,7 +231,7 @@ int gx_set_graph_batch_csr(gx_handle* h, int32_t num_graphs, int32_t max_nodes, 
 /* Plans the graphs to explain; edge_off[count+1] (may be NULL) receives the packed slot offsets: the slots of
  * graph t are the entries of its adjacency in row-major order (its slice of the CSR).  Any model gx_set_model accepts:
  * the default model needs every graph to fit the tuned kernel's shared memory (GX_ERR_UNSUPPORTED otherwise); a model
- * variant (2 or 4 .. 7 layers, --bn, widths 33..128) keeps each graph in device memory, bounded by max_nodes <= 4096 only. */
+ * variant (2 or 4 .. 7 layers, --bn, widths 33..256) keeps each graph in device memory, bounded by max_nodes <= 4096 only. */
 int gx_plan_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int64_t* edge_off, int64_t* total_edges);
 /* Explainer.explain(node_idx=0, graph_idx=g, graph_mode=True) for every planned graph (model =
  * GcnEncoderGraph: per-layer max-pool readout, models.py:269-316; lap_loss = 0, explain.py:787-788).
@@ -243,8 +247,9 @@ int gx_explain_graphs_ex(gx_handle* h, const gx_hparams* hp, gx_memspace space, 
  * explain.py:688-692) for every planned node (after gx_plan_nodes) or graph (after gx_plan_graphs).  The forward sees the dense
  * mask sym(sigmoid(M)) * (1 - I), NOT multiplied by the sub-adjacency, and the unmasked features; the loss (explain.py:740-808) is
  * evaluated on that dense matrix.  One CTA per task keeps its n^2 mask parameters in device memory: n = the k-hop set (node mode)
- * or max_nodes (graph mode), n > 4096 gives GX_ERR_UNSUPPORTED.  Every model and optimiser / scheduler of gx_hparams;
- * GX_INIT_STATE gives GX_ERR_UNSUPPORTED.  All buffers in `space`:
+ * or max_nodes (graph mode), n > 4096 gives GX_ERR_UNSUPPORTED.  Every optimiser / scheduler of gx_hparams and every model except
+ * attention models, inputs wider than 128 and hidden / output widths above 128 (GX_ERR_UNSUPPORTED); GX_INIT_STATE gives
+ * GX_ERR_UNSUPPORTED.  All buffers in `space`:
  *   m0_dense    [sum_t n_t^2] GX_INIT_M0: the full (n_t, n_t) M0 of every task, task after task (GX_INIT_PHILOX: NULL; the draw uses
  *               slot = i * n_t + j)
  *   edge_mask   [total_edges] out: masked_adj at the sub-adjacency slots (node mode: the sub_col slots; graph mode: the graph's

@@ -120,6 +120,34 @@ def main():
             eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=3), None, out)
             print("var ok deep graph", L, hid, bn, att, float(out.sum()))
             eng.close()
+        # hidden / output widths 129 .. 256 (explain_var.cu's row-block path): 256 / 256 with --bn, 160 / 136 on the wide input path
+        # (d = 300), node mode (hub and small tasks) with the model forward, and graph mode
+        for L, hid, emb, bn, d in ((3, 256, 256, True, d0), (4, 160, 136, False, 300)):
+            dims = [d] + [hid] * (L - 1) + [emb]
+            w = {}
+            for l in range(1, L + 1):
+                w["W%d" % l] = sc(dims[l - 1], dims[l]) / np.sqrt(dims[l - 1]); w["b%d" % l] = sc(dims[l])
+            w["Wp"], w["bp"] = sc(3, hid * (L - 1) + emb), sc(3)
+            feat = g["feat"].astype(np.float32) if d == d0 else rng.normal(size=(N, d)).astype(np.float32)
+            eng = gnnx.Engine(0)
+            eng.set_model(w, num_layers=L, bn=bn)
+            eng.set_graph_csr(rowptr, col, feat, g["label"].astype(np.int32), np.zeros(N, np.int32))
+            plan = eng.plan_nodes([0, 17], L)
+            out = np.zeros(plan.total_edges, np.float32)
+            eng.explain_nodes_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=2), None, out)
+            pred = eng.model_forward()
+            print("var ok wide layers node", L, hid, emb, bn, d, float(out.sum()), float(pred.sum()))
+            eng.close()
+            wg = dict(w)
+            wg["W1"] = sc(gg["feat"].shape[2], hid)
+            eng = gnnx.Engine(0)
+            eng.set_model(wg, num_layers=L, bn=bn)
+            eng.set_graph_batch(gg["adj"], gg["feat"], gg["label"] % 3)
+            eoff = eng.plan_graphs([0, 3, 5])
+            out = np.zeros(int(eoff[-1]), np.float32)
+            eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=3), None, out)
+            print("var ok wide layers graph", L, hid, emb, bn, float(out.sum()))
+            eng.close()
     if "cluster" in which:
         eng = util.make_engine(fx)
         eng.debug_cluster(4, 1)
