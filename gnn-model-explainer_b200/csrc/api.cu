@@ -203,11 +203,11 @@ int place_pair_slabs(gx_handle* h, GxExplainLaunch* cfg, const int* slabs, int n
 }
 
 int launch_var_batch(gx_handle* h, const char* who, int graph_mode, const GxHparamsDev& hd, const IoDev& D) {
-  const int bytes = gx_var_smem_bytes(graph_mode, h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C, h->m.att);
+  const int bytes = gx_var_smem_bytes(graph_mode, h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C, h->m.att, h->head);
   if (bytes > gx_explain_max_smem()) { gx_set_error("%s: model does not fit the variant kernel", who); return GX_ERR_UNSUPPORTED; }
   int max_ctas = h->num_sms * 4;
   if (graph_mode) {   // graph mode: as many CTAs as are co-resident
-    const int per_sm = gx_var_ctas_per_sm(graph_mode, h->m);
+    const int per_sm = gx_var_ctas_per_sm(graph_mode, h->m, h->head);
     if (per_sm < 1) { gx_set_error("%s: the variant kernel cannot be resident (%d bytes of shared memory)", who, bytes); return GX_ERR_UNSUPPORTED; }
     max_ctas = h->num_sms * per_sm;
   }
@@ -219,19 +219,21 @@ int launch_var_batch(gx_handle* h, const char* who, int graph_mode, const GxHpar
   if (rc == GX_OK) rc = place_pair_slabs(h, &cfg, &cfg.grid, 1);
   if (rc == GX_OK) rc = begin_timing(h);
   if (rc != GX_OK) return rc;
-  GX_CUDA_CHECK(gx_launch_explain_var(cfg, graph_mode, h->g, h->gb, h->m, hd, h->plan, D.m0, D.out, D.feat, h->stream));
+  GX_CUDA_CHECK(gx_launch_explain_var(cfg, graph_mode, h->g, h->gb, h->m, h->head, hd, h->plan, D.m0, D.out, D.feat, h->stream));
   h->launches += 1;
   return GX_OK;
 }
 
 // Model variant (num_gc_layers 2 / 4 .. 7, --bn, widths 33..256, attention, inputs wider than 128): explain_var.cu, true widths (a zero-padded column would enter
 // the bn statistics).  att_w != nullptr: an attention model, each layer's (in, in) attention weights right after its conv weights
-// (gx_att_weight).  The widths were checked by the caller.
+// (gx_att_weight).  head.k > 0: an MLP prediction head, whose Linears replace pred_w / pred_b (head_w / head_b: head.k + 1 pointers each),
+// its block after the conv layers (GxHeadDev).  The widths were checked by the caller.
 static int set_variant_model(gx_handle* h, const char* who, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
-                             const float* const* att_w, const float* pred_w, const float* pred_b) {
+                             const float* const* att_w, const float* pred_w, const float* pred_b, GxHeadDev head = GxHeadDev{},
+                             const float* const* head_w = nullptr, const float* const* head_b = nullptr) {
   const int L = dims->num_layers, d = dims->input_dim, hid0 = dims->hidden_dim, emb0 = dims->embed_dim, C = dims->num_classes;
   const int att = att_w != nullptr ? 1 : 0;
-  if (gx_var_smem_bytes(0, d, L, hid0, emb0, C, att) > gx_explain_max_smem()) {
+  if (gx_var_smem_bytes(0, d, L, hid0, emb0, C, att, head) > gx_explain_max_smem()) {
     gx_set_error("%s: model variant does not fit shared memory", who);
     return GX_ERR_UNSUPPORTED;
   }
@@ -249,10 +251,23 @@ static int set_variant_model(gx_handle* h, const char* who, const gx_model_dims*
     for (int c = 0; c < wout; ++c) host.push_back((conv_b && conv_b[l]) ? conv_b[l][c] : 0.f);
   }
   const int PD0 = hid0 * (L - 1) + emb0;
-  al4(); const size_t offWp = host.size();
-  host.insert(host.end(), pred_w, pred_w + (size_t)C * PD0);
-  al4(); const size_t offbp = host.size();
-  host.insert(host.end(), pred_b, pred_b + C);
+  al4();
+  size_t offWp = host.size(), offbp;
+  if (head.k == 0) {
+    host.insert(host.end(), pred_w, pred_w + (size_t)C * PD0);
+    al4(); offbp = host.size();
+    host.insert(host.end(), pred_b, pred_b + C);
+  } else {   // Linear j: weight then bias, back to back (gx_head_off); Wp / bp point at the last one
+    for (int j = 0; j <= head.k; ++j) {
+      const int in = gx_head_in(head, PD0, j), out = gx_head_out(head, C, j);
+      if (!head_w[j] || !head_b[j]) { gx_set_error("%s: head_w[%d] or head_b[%d] is NULL", who, j, j); return GX_ERR_INVALID; }
+      offWp = host.size();
+      host.insert(host.end(), head_w[j], head_w[j] + (size_t)out * in);
+      offbp = host.size();
+      host.insert(host.end(), head_b[j], head_b[j] + out);
+    }
+  }
+  const size_t offHead = host.size() - gx_head_words(head, PD0, C);
   GX_CUDA_CHECK(h->m_buf.reserve(host.size() * 4));
   GX_CUDA_CHECK(cudaMemcpyAsync(h->m_buf.p, host.data(), host.size() * 4, cudaMemcpyHostToDevice, h->stream));
   GX_CUDA_CHECK(cudaStreamSynchronize(h->stream));
@@ -262,6 +277,8 @@ static int set_variant_model(gx_handle* h, const char* who, const gx_model_dims*
   h->m.bn = (dims->flags & GX_MODEL_BN) ? 1 : 0; h->m.variant = 1; h->m.att = att;
   for (int l = 0; l < L; ++l) { h->m.W[l] = b + offW[l]; h->m.Wt[l] = nullptr; h->m.b[l] = b + offb[l]; }
   h->m.Wp = b + offWp; h->m.bp = b + offbp;
+  h->head = head;
+  h->head.W = head.k > 0 ? b + offHead : nullptr;
   h->has_model = true; h->has_plan = false;
   return GX_OK;
 }
@@ -436,12 +453,14 @@ int gx_model_forward(gx_handle* h, gx_memspace space, float* pred) {
   const size_t np_ = (size_t)h->g.N * h->m.C;
   const size_t nh = (size_t)h->m.L * h->g.N * gx_var_row_stride(h->m.hid, h->m.emb);   // every layer's rows, 32 / 64 / 128 / 256 floats each
   const size_t npw = h->m.att ? (size_t)h->g.N * gx_round_up(std::max(h->m.d, h->m.hid), 4) : 0;   // attention models: P
-  GX_CUDA_CHECK(h->d_fwd.reserve((nh + np_ + npw) * 4));
+  const size_t ne = h->head.k > 0 ? (size_t)h->g.N * (h->m.hid * (h->m.L - 1) + h->m.emb) : 0;   // MLP head: the concatenated rows
+  GX_CUDA_CHECK(h->d_fwd.reserve((nh + np_ + npw + ne) * 4));
   float* H = h->d_fwd.as<float>();
   float* pd = space == GX_DEVICE ? pred : H + nh;
   float* P = h->m.att ? H + nh + np_ : nullptr;
-  GX_CUDA_CHECK(gx_launch_model_forward(h->g, h->m, H, pd, nullptr, P, h->stream));
-  h->launches += h->m.L * (h->m.att ? 2 : 1) + 1;
+  float* E = h->head.k > 0 ? H + nh + np_ + npw : nullptr;
+  GX_CUDA_CHECK(gx_launch_model_forward(h->g, h->m, h->head, H, pd, E, P, h->stream));
+  h->launches += h->m.L * (h->m.att ? 2 : 1) + 1 + (h->head.k > 0 ? 1 : 0);
   if (space != GX_DEVICE) {
     GX_CUDA_CHECK(cudaMemcpyAsync(pred, pd, np_ * 4, cudaMemcpyDeviceToHost, h->stream));
     GX_CUDA_CHECK(cudaStreamSynchronize(h->stream));
@@ -529,6 +548,7 @@ int gx_set_model(gx_handle* h, const gx_model_dims* dims, const float* const* co
   for (int l = 0; l < 3; ++l) { h->m.W[l] = b + offW[l]; h->m.Wt[l] = b + offWt[l]; h->m.b[l] = b + offb[l]; }
   h->m.Wp = b + offWp;
   h->m.bp = b + offbp;
+  h->head = GxHeadDev{};
   h->has_model = true;
   h->has_plan = false;
   return GX_OK;
@@ -550,6 +570,38 @@ int gx_set_model_att(gx_handle* h, const gx_model_dims* dims, const float* const
   }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
   return set_variant_model(h, "gx_set_model_att", dims, conv_w, conv_b, att_w, pred_w, pred_b);
+}
+
+int gx_set_model_head(gx_handle* h, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
+                      const float* const* att_w, int32_t head_layers, const int32_t* head_widths, const float* const* head_w,
+                      const float* const* head_b) {
+  const char* who = "gx_set_model_head";
+  if (!h || !dims || !conv_w || !head_widths || !head_w || !head_b) { gx_set_error("%s: NULL argument", who); return GX_ERR_INVALID; }
+  const int rc = check_model_dims(who, dims);
+  if (rc != GX_OK) return rc;
+  if (head_layers < 1 || head_layers > GX_MAX_HEAD_LAYERS) {
+    gx_set_error("%s: head_layers=%d outside [1,%d] (GX_MAX_HEAD_LAYERS; a model without hidden head layers is set with gx_set_model)", who,
+                 head_layers, GX_MAX_HEAD_LAYERS);
+    return GX_ERR_UNSUPPORTED;
+  }
+  GxHeadDev head{};
+  head.k = head_layers;
+  for (int j = 0; j < head_layers; ++j) {
+    if (head_widths[j] < 1 || head_widths[j] > GX_MAX_WIDTH) {
+      gx_set_error("%s: head_widths[%d]=%d outside [1,%d] (GX_MAX_WIDTH)", who, j, head_widths[j], GX_MAX_WIDTH);
+      return GX_ERR_UNSUPPORTED;
+    }
+    head.w[j] = head_widths[j];
+  }
+  const bool att = att_w != nullptr;
+  if ((dims->flags & GX_MODEL_ATT) && !att) { gx_set_error("%s: GX_MODEL_ATT without att_w", who); return GX_ERR_INVALID; }
+  if (att && (dims->input_dim >= GX_VAR_WIDE_MIN || dims->hidden_dim > 128 || dims->embed_dim > 128)) {
+    gx_set_error("%s: input_dim=%d hidden_dim=%d output_dim=%d; attention models are built for inputs and widths up to 128", who, dims->input_dim,
+                 dims->hidden_dim, dims->embed_dim);
+    return GX_ERR_UNSUPPORTED;
+  }
+  GX_CUDA_CHECK(cudaSetDevice(h->device));
+  return set_variant_model(h, who, dims, conv_w, conv_b, att_w, nullptr, nullptr, head, head_w, head_b);
 }
 
 int gx_set_graph_csr(gx_handle* h, int64_t N, const int32_t* rowptr, const int32_t* col,

@@ -31,13 +31,14 @@ struct DenseArgs {
   GxHparamsDev hp;
   GxPlanArrays plan;
   GxDenseIo io;
+  GxHeadDev hd;   // MLP prediction head (k = 0: none)
 };
 
 // shared memory: the variant kernels' carve-up + the arg-max row of every pooled feature (graph mode) + reduction scratch
 struct DenseSmem { VarSmem S; int arg, red, total; };
-__host__ __device__ inline DenseSmem dense_smem(int d, int L, int hid, int emb, int C, int nwarps) {
+__host__ __device__ inline DenseSmem dense_smem(int d, int L, int hid, int emb, int C, int nwarps, const GxHeadDev& hd) {
   DenseSmem D;
-  D.S = var_smem(d, L, hid, emb, C, nwarps);
+  D.S = var_smem(d, L, hid, emb, C, nwarps, 0, hd);
   const int PD = hid * (L - 1) + emb;
   D.arg = D.S.total;
   D.red = D.arg + gx_round_up(PD, 4);
@@ -119,14 +120,15 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
   const int dp = gx_round_up(d, 4);
   const int PD = hid * (L - 1) + embw;
   const bool ieee = (hp.flags & GX_HP_IEEE_EDGE) != 0;
-  const DenseSmem DS = dense_smem(d, L, hid, embw, C, nwarps);
+  const GxHeadDev& hd = A.hd;
+  const DenseSmem DS = dense_smem(d, L, hid, embw, C, nwarps, hd);
   const VarSmem& S = DS.S;
   float* const sF = sm + S.sF; float* const Fm = sm + S.F; float* const mF = sm + S.mF; float* const vF = sm + S.vF;
   float* const zs = sm + S.zs + warp * S.zlen;
   float* const emb = sm + S.emb; float* const dEmb = sm + S.dEmb; float* const logit = sm + S.logit;
   int* const arg = reinterpret_cast<int*>(sm + DS.arg);
   double* const red = reinterpret_cast<double*>(sm + DS.red);
-  const bool wp_smem = C * (PD + 1) <= GX_WP_SMEM_MAX;
+  const bool wp_smem = gx_head_words(hd, PD, C) <= GX_WP_SMEM_MAX;
   const float* const Wpp = wp_smem ? sm + S.Wp : m.Wp;
   const float* const bpp = wp_smem ? sm + S.Wp + C * PD : m.bp;
   auto win_of = [&](int l) { return l == 0 ? d : hid; };            // l = 0 .. L-1
@@ -142,7 +144,7 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
   };
 
   const float* Wl[GX_MAX_LAYERS];   // conv weights: shared memory when they fit, else global (L2 resident)
-  var_stage_model(m, S, sm, Wl, tid, NT);
+  var_stage_model(m, hd, S, sm, Wl, tid, NT);
   float* const slab = A.gws + (int64_t)blockIdx.x * A.gws_stride_words;
 
   for (;;) {
@@ -234,9 +236,9 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
           for (int c = lane; c < wout_of(l - 1); c += 32) emb[hid * (l - 1) + c] = Hc[(int64_t)r * KH + off(l) + c];
       }
       __syncthreads();
+      var_readout_tail(emb, hd, wp_smem ? sm + S.Wp : hd.W, Wpp, bpp, C, PD, gt, sm + S.hx, sm + S.hg, logit, dEmb, tid, NT);
+      __syncthreads();
       if (warp == 0) {
-        var_readout_tail(emb, Wpp, bpp, C, PD, gt, logit, dEmb, lane);
-        __syncwarp();
         if (lane == 0) s_pgt = logit[gt] + 1.f;
         if (io.trace_pred != nullptr)
           for (int c = lane; c < C; c += 32) io.trace_pred[((int64_t)task_id * io.epochs + (it - 1)) * C + c] = logit[c] + (c == gt ? 1.f : 0.f);
@@ -349,24 +351,24 @@ __global__ void __launch_bounds__(kVarThreads) explain_dense_kernel(const DenseA
 
 }  // namespace
 
-int gx_dense_smem_bytes(int d, int L, int hid, int emb, int C) { return dense_smem(d, L, hid, emb, C, kVarThreads / 32).total * 4; }
+int gx_dense_smem_bytes(int d, int L, int hid, int emb, int C, const GxHeadDev& hd) { return dense_smem(d, L, hid, emb, C, kVarThreads / 32, hd).total * 4; }
 
 // co-resident CTAs per SM of the model's instantiation (sizes the persistent grid); 0 on error
-int gx_dense_ctas_per_sm(const GxModelDev& m) {
-  const int bytes = gx_dense_smem_bytes(m.d, m.L, m.hid, m.emb, m.C);
+int gx_dense_ctas_per_sm(const GxModelDev& m, const GxHeadDev& hd) {
+  const int bytes = gx_dense_smem_bytes(m.d, m.L, m.hid, m.emb, m.C, hd);
   int n = 0;
   var_dispatch(m, [&](auto bn, auto kw) { n = var_ctas_per_sm(explain_dense_kernel<decltype(bn)::value, decltype(kw)::value>, bytes); return cudaSuccess; });
   return n;
 }
 
 cudaError_t gx_launch_explain_dense(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
-                                    const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan, const GxDenseIo& io,
-                                    cudaStream_t s) {
+                                    const GxModelDev& m, const GxHeadDev& hd, const GxHparamsDev& hp, const GxPlanArrays& plan,
+                                    const GxDenseIo& io, cudaStream_t s) {
   DenseArgs args;
   args.order = cfg.order; args.ntasks = cfg.ntasks; args.counter = cfg.counter;
   args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
-  args.graph_mode = graph_mode; args.g = g; args.gb = gb; args.m = m; args.hp = hp; args.plan = plan; args.io = io;
-  const int bytes = gx_dense_smem_bytes(m.d, m.L, m.hid, m.emb, m.C);
+  args.graph_mode = graph_mode; args.g = g; args.gb = gb; args.m = m; args.hp = hp; args.plan = plan; args.io = io; args.hd = hd;
+  const int bytes = gx_dense_smem_bytes(m.d, m.L, m.hid, m.emb, m.C, hd);
   return var_dispatch(m, [&](auto bn, auto kw) {
     return var_launch(explain_dense_kernel<decltype(bn)::value, decltype(kw)::value>, args, cfg.grid, bytes, s);
   });

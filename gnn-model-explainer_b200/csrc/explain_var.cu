@@ -60,6 +60,7 @@ struct VarArgs {
   const float* m0;
   float* out_mask;
   float* out_feat;
+  GxHeadDev hd;          // MLP prediction head (k = 0: none)
 };
 
 // ---------------------------------------------------------------------------------------------------------------- attention layers
@@ -243,21 +244,22 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
   const int dp = gx_round_up(d, 4);
   const int PD = hid * (L - 1) + embw;
   const bool ieee = (hp.flags & GX_HP_IEEE_EDGE) != 0;
-  const VarSmem S = var_smem_of<kWide>(d, L, hid, embw, C, nwarps, kAtt ? 1 : 0);
+  const GxHeadDev& hd = A.hd;
+  const VarSmem S = var_smem_of<kWide>(d, L, hid, embw, C, nwarps, kAtt ? 1 : 0, hd);
   float* const sF = sm + S.sF; float* const Fm = sm + S.F; float* const mF = sm + S.mF; float* const vF = sm + S.vF;
   float* const zs = sm + S.zs + warp * S.zlen;
   float* const gFp = sm + S.gFp;
   float* const emb = sm + S.emb; float* const dEmb = sm + S.dEmb; float* const logit = sm + S.logit;
   float* const cst = sm + S.total;                                              // graph mode (gx_var_smem_bytes)
   int* const arg = reinterpret_cast<int*>(sm + S.total + gx_round_up(PD, 4));   // graph mode
-  const bool wp_smem = C * (PD + 1) <= GX_WP_SMEM_MAX;
+  const bool wp_smem = gx_head_words(hd, PD, C) <= GX_WP_SMEM_MAX;
   const float* const Wpp = wp_smem ? sm + S.Wp : m.Wp;
   const float* const bpp = wp_smem ? sm + S.Wp + C * PD : m.bp;
   auto win_of = [&](int l) { return l == 0 ? d : hid; };            // l = 0 .. L-1
   auto wout_of = [&](int l) { return l == L - 1 ? embw : hid; };
 
   const float* Wl[GX_MAX_LAYERS];   // conv weights: shared memory when they fit, else global (L2 resident)
-  var_stage_model<kWide>(m, S, sm, Wl, tid, NT);
+  var_stage_model<kWide>(m, hd, S, sm, Wl, tid, NT);
   const float* Wal[kAtt ? GX_MAX_LAYERS : 1];  // attention weights (kAtt), staged like Wl
   if constexpr (kAtt) var_stage_att(m, S, sm, Wal, tid, NT);
   if constexpr (kGraph) {
@@ -425,14 +427,13 @@ __global__ void __launch_bounds__(kVarThreads, kGraph ? (KW == 1 && !kBn ? 2 : 1
         var_max_pool(L, hid, PD, n, Hh, VW, (Tp->flags & 1) != 0 ? cst : nullptr, -1, emb, arg, tid, NT);
         __syncthreads();
       }
-      if (warp == 0) {
-        if constexpr (!kGraph) {   // node mode reads out row r = level-order id 0
+      if constexpr (!kGraph) {   // node mode reads out row r = level-order id 0
+        if (warp == 0)
           for (int l = 1; l <= L; ++l)
             for (int c = lane; c < wout_of(l - 1); c += 32) emb[hid * (l - 1) + c] = Hh(l)[c];
-          __syncwarp();
-        }
-        var_readout_tail(emb, Wpp, bpp, C, PD, gt, logit, dEmb, lane);
+        __syncthreads();
       }
+      var_readout_tail(emb, hd, wp_smem ? sm + S.Wp : hd.W, Wpp, bpp, C, PD, gt, sm + S.hx, sm + S.hg, logit, dEmb, tid, NT);
       if constexpr (!kWide)
         for (int idx = tid; idx < nwarps * dp; idx += NT) gFp[idx] = 0.f;
       __syncthreads();
@@ -658,27 +659,27 @@ cudaError_t with_var_kernel(int graph_mode, const GxModelDev& m, F&& f) {
 }  // namespace
 
 // var_smem's carve-up + in graph mode the edge-less rows' constant embedding and the arg-max row of every pooled feature (cst, arg)
-int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C, int att) {
+int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C, int att, const GxHeadDev& hd) {
   const int pool = graph_mode ? 2 * gx_round_up(hid * (L - 1) + emb, 4) : 0;
-  const int words = d >= GX_VAR_WIDE_MIN ? var_smem_wide(d, L, hid, emb, C, kVarThreads / 32).total
-                                         : var_smem(d, L, hid, emb, C, kVarThreads / 32, att).total;
+  const int words = d >= GX_VAR_WIDE_MIN ? var_smem_wide(d, L, hid, emb, C, kVarThreads / 32, hd).total
+                                         : var_smem(d, L, hid, emb, C, kVarThreads / 32, att, hd).total;
   return (words + pool) * 4;
 }
 int gx_var_row_stride(int hid, int emb) { return 32 * var_row_kw(hid, emb); }
 
-int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m) {
-  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C, m.att);
+int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m, const GxHeadDev& hd) {
+  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C, m.att, hd);
   int n = 0;
   with_var_kernel(graph_mode, m, [&](auto kern) { n = var_ctas_per_sm(kern, bytes); return cudaSuccess; });
   return n;
 }
 
 cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
-                                  const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
+                                  const GxModelDev& m, const GxHeadDev& hd, const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                   float* out_mask, float* out_feat, cudaStream_t s) {
   VarArgs args;
   fill_queue_args(args, cfg, m, hp, plan, m0, out_mask, out_feat);
-  args.g = g; args.gb = gb; args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words;
-  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C, m.att);
+  args.g = g; args.gb = gb; args.gws = cfg.gws; args.gws_stride_words = cfg.gws_stride_words; args.hd = hd;
+  const int bytes = gx_var_smem_bytes(graph_mode, m.d, m.L, m.hid, m.emb, m.C, m.att, hd);
   return with_var_kernel(graph_mode, m, [&](auto kern) { return var_launch(kern, args, cfg.grid, bytes, s); });
 }

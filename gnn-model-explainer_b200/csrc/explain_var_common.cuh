@@ -23,7 +23,9 @@ inline int var_row_kw(int hid, int emb) { return (hid > emb ? hid : emb) > 128 ?
 // state, per-warp scratch rows and partial dL/dsF, the readout vectors.  Attention models (att != 0) also stage the (in, in)
 // attention weights when they fit the weight budget together with the conv weights (var_att_in_smem): the last var_att_words words
 // before S.total, layer by layer; else they are read through L2 and the conv weights are staged as for any other model.
-struct VarSmem { int W[GX_MAX_LAYERS], b[GX_MAX_LAYERS], Wp, sF, F, mF, vF, zs, zlen, gFp, emb, dEmb, logit, w_in_smem, total; };
+// Models with an MLP prediction head (hd.k > 0) also hold the head's activations hx (its widths back to back) and two gradient
+// vectors hg of its largest width; pred_model's slot Wp holds the whole head block when it fits.  Head-less models: zero words.
+struct VarSmem { int W[GX_MAX_LAYERS], b[GX_MAX_LAYERS], Wp, sF, F, mF, vF, zs, zlen, gFp, emb, dEmb, logit, hx, hg, w_in_smem, total; };
 __host__ __device__ inline int var_att_words(int d, int L, int hid) {
   int w = 0;
   for (int l = 0; l < L; ++l) w += gx_round_up((l == 0 ? d : hid) * (l == 0 ? d : hid), 4);
@@ -37,7 +39,7 @@ __host__ __device__ inline int var_conv_words(int d, int L, int hid, int emb) {
 __host__ __device__ inline bool var_att_in_smem(int d, int L, int hid, int emb) {
   return var_conv_words(d, L, hid, emb) + var_att_words(d, L, hid) <= kVarWeightWords;
 }
-__host__ __device__ inline VarSmem var_smem(int d, int L, int hid, int emb, int C, int nwarps, int att = 0) {
+__host__ __device__ inline VarSmem var_smem(int d, int L, int hid, int emb, int C, int nwarps, int att = 0, const GxHeadDev& hd = GxHeadDev{}) {
   VarSmem S;
   const int dp = gx_round_up(d, 4);
   int o = 0;
@@ -51,12 +53,14 @@ __host__ __device__ inline VarSmem var_smem(int d, int L, int hid, int emb, int 
     S.b[l] = take(wout);
   }
   const int PD = hid * (L - 1) + emb;
-  S.Wp = take(C * (PD + 1) <= GX_WP_SMEM_MAX ? C * (PD + 1) : 0);
+  const int hw = gx_head_words(hd, PD, C);
+  S.Wp = take(hw <= GX_WP_SMEM_MAX ? hw : 0);
   S.sF = take(dp); S.F = take(dp); S.mF = take(dp); S.vF = take(dp);
   S.zlen = dp > 32 * var_kw(hid, emb) ? dp : 32 * var_kw(hid, emb);   // per-warp scratch row: a feature row or a hidden row
   S.zs = take(nwarps * S.zlen);
   S.gFp = take(nwarps * dp);
   S.emb = take(PD); S.dEmb = take(PD); S.logit = take(C < 32 ? 32 : C);
+  S.hx = take(gx_head_act_words(hd)); S.hg = take(2 * gx_head_max_width(hd));
   if (att && var_att_in_smem(d, L, hid, emb)) take(var_att_words(d, L, hid));
   S.total = o;
   return S;
@@ -65,7 +69,7 @@ __host__ __device__ inline VarSmem var_smem(int d, int L, int hid, int emb, int 
 // Wide inputs (d > 128, explain_var.cu kWide) keep the feature-mask state and layer 1's products in the task slab and read W1 through
 // L2, so that nothing here grows with d: no feature-mask arrays or dL/dsF partials, hidden-width scratch rows, and only the layers
 // >= 2 are staged (S.W[0] takes zero words).
-__host__ __device__ inline VarSmem var_smem_wide(int d, int L, int hid, int emb, int C, int nwarps) {
+__host__ __device__ inline VarSmem var_smem_wide(int d, int L, int hid, int emb, int C, int nwarps, const GxHeadDev& hd = GxHeadDev{}) {
   VarSmem S;
   int o = 0;
   auto take = [&](int words) { int r = o; o += gx_round_up(words, 4); return r; };
@@ -78,27 +82,30 @@ __host__ __device__ inline VarSmem var_smem_wide(int d, int L, int hid, int emb,
     S.b[l] = take(wout);
   }
   const int PD = hid * (L - 1) + emb;
-  S.Wp = take(C * (PD + 1) <= GX_WP_SMEM_MAX ? C * (PD + 1) : 0);
+  const int hw = gx_head_words(hd, PD, C);
+  S.Wp = take(hw <= GX_WP_SMEM_MAX ? hw : 0);
   S.sF = S.F = S.mF = S.vF = o;
   S.zlen = 32 * var_kw(hid, emb);
   S.zs = take(nwarps * S.zlen);
   S.gFp = o;
   S.emb = take(PD); S.dEmb = take(PD); S.logit = take(C < 32 ? 32 : C);
+  S.hx = take(gx_head_act_words(hd)); S.hg = take(2 * gx_head_max_width(hd));
   S.total = o;
   (void)d;
   return S;
 }
 template <bool kWide>
-__host__ __device__ inline VarSmem var_smem_of(int d, int L, int hid, int emb, int C, int nwarps, int att) {
-  if constexpr (kWide) return var_smem_wide(d, L, hid, emb, C, nwarps);
-  else return var_smem(d, L, hid, emb, C, nwarps, att);
+__host__ __device__ inline VarSmem var_smem_of(int d, int L, int hid, int emb, int C, int nwarps, int att, const GxHeadDev& hd) {
+  if constexpr (kWide) return var_smem_wide(d, L, hid, emb, C, nwarps, hd);
+  else return var_smem(d, L, hid, emb, C, nwarps, att, hd);
 }
 
-// Stages conv biases (always), conv weights (when S.w_in_smem) and pred_model (when small) in shared memory; Wl[l] = where layer l's
-// weights are read from.
+// Stages conv biases (always), conv weights (when S.w_in_smem) and pred_model or the MLP head block (when small) in shared memory;
+// Wl[l] = where layer l's weights are read from.
 // With kWide, layer 1's weights stay in global memory (var_smem_wide).
 template <bool kWide = false>
-__device__ __forceinline__ void var_stage_model(const GxModelDev& m, const VarSmem& S, float* sm, const float** Wl, int tid, int nt) {
+__device__ __forceinline__ void var_stage_model(const GxModelDev& m, const GxHeadDev& hd, const VarSmem& S, float* sm, const float** Wl, int tid,
+                                                int nt) {
   const int L = m.L, PD = m.hid * (L - 1) + m.emb;
   for (int l = 0; l < L; ++l) {
     if constexpr (kWide) {
@@ -115,7 +122,11 @@ __device__ __forceinline__ void var_stage_model(const GxModelDev& m, const VarSm
     Wl[l] = S.w_in_smem ? sm + S.W[l] : m.W[l];
     for (int idx = tid; idx < wout; idx += nt) sm[S.b[l] + idx] = __ldg(m.b[l] + idx);
   }
-  if (m.C * (PD + 1) <= GX_WP_SMEM_MAX) {
+  const int hw = gx_head_words(hd, PD, m.C);
+  if (hw > GX_WP_SMEM_MAX) return;
+  if (hd.k > 0) {
+    for (int idx = tid; idx < hw; idx += nt) sm[S.Wp + idx] = __ldg(hd.W + idx);
+  } else {
     for (int idx = tid; idx < m.C * PD; idx += nt) sm[S.Wp + idx] = __ldg(m.Wp + idx);
     for (int idx = tid; idx < m.C; idx += nt) sm[S.Wp + m.C * PD + idx] = __ldg(m.bp + idx);
   }
@@ -365,30 +376,61 @@ __device__ __forceinline__ void var_edge_update(const GxHparamsDev& hp, float g,
   }
 }
 
-// Readout tail shared by both modes (one warp): logits = Wp emb + bp, softmax, dL/dlogits = p - onehot(gt) (explain.py:750-753),
-// dEmb = Wp^T dL/dlogits.
-__device__ __forceinline__ void var_readout_tail(const float* emb, const float* Wpp, const float* bpp, int C, int PD, int gt, float* logit,
-                                                 float* dEmb, int lane) {
-  for (int c = 0; c < C; ++c) {
-    float t = 0.f;
-    for (int k = lane; k < PD; k += 32) t = fmaf(emb[k], Wpp[c * PD + k], t);
-    t = warp_sum(t);
-    if (lane == 0) logit[c] = t + bpp[c];
+// Readout tail shared by both modes and kernels (every thread calls; emb must be complete; the caller synchronises before reading
+// logit or dEmb).  pred_model = Linear 0 .. k of the head (k = 0: Wp / bp; else the head block blk, models.py:193-207):
+//   forward  x_0 = emb, x_j = relu(W_j x_{j-1} + b_j) into hx, logits = W_k x_k + b_k;  softmax, dL/dlogits = p - onehot(gt)
+//            (explain.py:750-753) into logit;
+//   backward g = W_j^T g, through each ReLU (0 where x_j <= 0, as torch) down to dEmb = W_0^T g.
+// Each output of a forward product is one warp's lane-strided dot and warp sum, each entry of a backward product one thread's chain over
+// the outputs in ascending order, whichever warp or thread takes it: a head-less model computes what one warp computed before.
+__device__ __forceinline__ void var_readout_tail(const float* emb, const GxHeadDev& hd, const float* blk, const float* Wpp, const float* bpp,
+                                                 int C, int PD, int gt, float* hx, float* hg, float* logit, float* dEmb, int tid, int nt) {
+  const int lane = tid & 31, warp = tid >> 5, nwarps = nt >> 5;
+  const int k = hd.k, mw = gx_head_max_width(hd);
+  auto lin = [&](int j, const float*& W, const float*& b) {   // Linear j's weight (out, in) and bias
+    if (k == 0) { W = Wpp; b = bpp; return; }
+    W = blk + gx_head_off(hd, PD, C, j);
+    b = W + gx_head_out(hd, C, j) * gx_head_in(hd, PD, j);
+  };
+  auto act = [&](int j) { int o = 0; for (int i = 0; i < j; ++i) o += hd.w[i]; return hx + o; };   // hidden layer j's output x_{j+1}
+  for (int j = 0; j <= k; ++j) {
+    const int in = gx_head_in(hd, PD, j), out = gx_head_out(hd, C, j);
+    const float *W, *b;
+    lin(j, W, b);
+    const float* const x = j == 0 ? emb : act(j - 1);
+    float* const y = j == k ? logit : act(j);
+    for (int o = warp; o < out; o += nwarps) {
+      float t = 0.f;
+      for (int i = lane; i < in; i += 32) t = fmaf(x[i], W[o * in + i], t);
+      t = warp_sum(t);
+      if (lane == 0) y[o] = j == k ? t + b[o] : fmaxf(t + b[o], 0.f);
+    }
+    __syncthreads();
   }
-  __syncwarp();
-  float mx = -INFINITY;
-  for (int c = lane; c < C; c += 32) mx = fmaxf(mx, logit[c]);
-  mx = warp_max(mx);
-  float se = 0.f;
-  for (int c = lane; c < C; c += 32) se += expf(logit[c] - mx);
-  se = warp_sum(se);
-  __syncwarp();
-  for (int c = lane; c < C; c += 32) logit[c] = expf(logit[c] - mx) / se - (c == gt ? 1.f : 0.f);
-  __syncwarp();
-  for (int k = lane; k < PD; k += 32) {
-    float t = 0.f;
-    for (int c = 0; c < C; ++c) t = fmaf(logit[c], Wpp[c * PD + k], t);
-    dEmb[k] = t;
+  if (warp == 0) {
+    float mx = -INFINITY;
+    for (int c = lane; c < C; c += 32) mx = fmaxf(mx, logit[c]);
+    mx = warp_max(mx);
+    float se = 0.f;
+    for (int c = lane; c < C; c += 32) se += expf(logit[c] - mx);
+    se = warp_sum(se);
+    __syncwarp();
+    for (int c = lane; c < C; c += 32) logit[c] = expf(logit[c] - mx) / se - (c == gt ? 1.f : 0.f);
+  }
+  __syncthreads();
+  for (int j = k; j >= 0; --j) {
+    const int in = gx_head_in(hd, PD, j), out = gx_head_out(hd, C, j);
+    const float *W, *b;
+    lin(j, W, b);
+    const float* const g = j == k ? logit : hg + (j & 1) * mw;
+    float* const dx = j == 0 ? dEmb : hg + ((j - 1) & 1) * mw;
+    const float* const xin = j == 0 ? nullptr : act(j - 1);
+    for (int i = tid; i < in; i += nt) {
+      float t = 0.f;
+      for (int o = 0; o < out; ++o) t = fmaf(g[o], W[o * in + i], t);
+      dx[i] = xin != nullptr && !(xin[i] > 0.f) ? 0.f : t;
+    }
+    if (j > 0) __syncthreads();
   }
 }
 

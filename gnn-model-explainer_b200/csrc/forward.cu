@@ -143,8 +143,38 @@ __global__ void __launch_bounds__(kFwdThreads) readout_kernel(int64_t N, int L, 
   }
 }
 
+// MLP prediction head (models.py:193-207) on every row: x_0 = emb_i, x_j = relu(W_j x_{j-1} + b_j), pred_i = W_k x_k + b_k, a warp per row
+// with the products of the explainer kernels' readout tail (each output a lane-strided dot and a warp sum), x_j in two per-warp vectors
+// of the head's largest width.
+__global__ void __launch_bounds__(kFwdThreads) head_kernel(int64_t N, int PD, int C, GxHeadDev hd, const float* __restrict__ emb,
+                                                           float* __restrict__ pred) {
+  extern __shared__ float xs_all[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = kFwdThreads / 32;
+  const int mw = gx_head_max_width(hd);
+  float* const xs = xs_all + warp * 2 * mw;
+  for (int64_t i = (int64_t)blockIdx.x * nwarps + warp; i < N; i += (int64_t)gridDim.x * nwarps) {
+    for (int j = 0; j <= hd.k; ++j) {
+      const int in = gx_head_in(hd, PD, j), out = gx_head_out(hd, C, j);
+      const float* const W = hd.W + gx_head_off(hd, PD, C, j);
+      const float* const b = W + out * in;
+      const float* const x = j == 0 ? emb + i * PD : xs + ((j - 1) & 1) * mw;
+      for (int o = 0; o < out; ++o) {
+        float t = 0.f;
+        for (int f = lane; f < in; f += 32) t = fmaf(x[f], __ldg(W + o * in + f), t);
+        t = warp_sum(t);
+        if (lane == 0) {
+          if (j == hd.k) pred[i * C + o] = t + __ldg(b + o);
+          else xs[(j & 1) * mw + o] = fmaxf(t + __ldg(b + o), 0.f);
+        }
+      }
+      __syncwarp();
+    }
+  }
+}
+
 template <int KW>
-cudaError_t model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, float* pred, float* emb_out, float* P, cudaStream_t s) {
+cudaError_t model_forward(const GxGraphDev& g, const GxModelDev& m, const GxHeadDev& hd, float* H, float* pred, float* emb_out, float* P,
+                          cudaStream_t s) {
   constexpr int LD = 32 * KW;
   const int nwarps = kFwdThreads / 32;
   const int grid = (int)std::min<int64_t>((g.N + nwarps - 1) / nwarps, GX_GRID_CAP);
@@ -166,19 +196,28 @@ cudaError_t model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, fl
     if (l == 0) gcn_layer_kernel<true, false, KW><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, nullptr, Hout);
     else gcn_layer_kernel<false, false, KW><<<grid, kFwdThreads, smem, s>>>(g, Hin, m.W[l], m.b[l], win, wout, l == m.L - 1, m.bn, nullptr, Hout);
   }
-  readout_kernel<KW><<<grid, kFwdThreads, 0, s>>>(g.N, m.L, m.hid, m.emb, m.C, H, m.Wp, m.bp, pred, emb_out);
+  if (hd.k == 0) {
+    readout_kernel<KW><<<grid, kFwdThreads, 0, s>>>(g.N, m.L, m.hid, m.emb, m.C, H, m.Wp, m.bp, pred, emb_out);
+    return cudaGetLastError();
+  }
+  // head models: the concatenated rows into emb_out (no pred_model product: C = 0), then the head
+  readout_kernel<KW><<<grid, kFwdThreads, 0, s>>>(g.N, m.L, m.hid, m.emb, 0, H, nullptr, nullptr, nullptr, emb_out);
+  head_kernel<<<grid, kFwdThreads, (size_t)nwarps * 2 * gx_head_max_width(hd) * sizeof(float), s>>>(g.N, m.hid * (m.L - 1) + m.emb, m.C, hd,
+                                                                                                      emb_out, pred);
   return cudaGetLastError();
 }
 
 }  // namespace
 
 // H: workspace [L][N][gx_var_row_stride(hid, emb)] floats (device).  Layer 1 keeps one input row per warp in dynamic shared memory: 128 KB
-// at the widest input (d = 4096), beyond the 48 KB a launch gets without opting in.  pred [N][C], emb_out [N][PD] or nullptr (device).
-// P: attention models' workspace [N][round_up(max(d, hid), 4)] floats (device), else unused.
-cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, float* pred, float* emb_out, float* P, cudaStream_t s) {
+// at the widest input (d = 4096), beyond the 48 KB a launch gets without opting in.  pred [N][C], emb_out [N][PD] or nullptr (device;
+// required with an MLP head, hd.k > 0).  P: attention models' workspace [N][round_up(max(d, hid), 4)] floats (device), else unused.
+cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, const GxHeadDev& hd, float* H, float* pred, float* emb_out, float* P,
+                                    cudaStream_t s) {
+  if (hd.k > 0 && emb_out == nullptr) return cudaErrorInvalidValue;
   const int kw = gx_var_row_stride(m.hid, m.emb) / 32;
-  if (kw == 1) return model_forward<1>(g, m, H, pred, emb_out, P, s);
-  if (kw == 2) return model_forward<2>(g, m, H, pred, emb_out, P, s);
-  if (kw == 4) return model_forward<4>(g, m, H, pred, emb_out, P, s);
-  return model_forward<8>(g, m, H, pred, emb_out, P, s);
+  if (kw == 1) return model_forward<1>(g, m, hd, H, pred, emb_out, P, s);
+  if (kw == 2) return model_forward<2>(g, m, hd, H, pred, emb_out, P, s);
+  if (kw == 4) return model_forward<4>(g, m, hd, H, pred, emb_out, P, s);
+  return model_forward<8>(g, m, hd, H, pred, emb_out, P, s);
 }

@@ -84,6 +84,27 @@ __host__ __device__ inline const float* gx_att_weight(const GxModelDev& m, int l
   return m.W[l] + (l == 0 ? m.d : m.hid) * (l == m.L - 1 ? m.emb : m.hid);
 }
 
+// MLP prediction head (gx_set_model_head, models.py:193-207): k hidden Linear + ReLU layers of widths w[0 .. k-1], then Linear(., C).
+// The k + 1 Linears lie back to back at W, each as its row-major (out, in) weight followed by its out biases, so that the head is one
+// block (staged in shared memory with one copy when it fits).  k = 0: no head, pred_model is GxModelDev's Wp / bp.  A separate kernel
+// argument of the variant, dense and forward kernels: GxModelDev is also an argument of the tuned kernels, which never see a head.
+struct GxHeadDev {
+  int32_t k;
+  int32_t w[GX_MAX_HEAD_LAYERS];
+  const float* W;
+};
+__host__ __device__ inline int gx_head_in(const GxHeadDev& hd, int PD, int j) { return j == 0 ? PD : hd.w[j - 1]; }
+__host__ __device__ inline int gx_head_out(const GxHeadDev& hd, int C, int j) { return j == hd.k ? C : hd.w[j]; }
+// words of Linear 0 .. j-1 in the block (j = k + 1: the whole head; k = 0: C (PD + 1), pred_model's weight and bias)
+__host__ __device__ inline int gx_head_off(const GxHeadDev& hd, int PD, int C, int j) {
+  int o = 0;
+  for (int i = 0; i < j; ++i) o += gx_head_out(hd, C, i) * (gx_head_in(hd, PD, i) + 1);
+  return o;
+}
+__host__ __device__ inline int gx_head_words(const GxHeadDev& hd, int PD, int C) { return gx_head_off(hd, PD, C, hd.k + 1); }
+__host__ __device__ inline int gx_head_act_words(const GxHeadDev& hd) { int s = 0; for (int j = 0; j < hd.k; ++j) s += hd.w[j]; return s; }
+__host__ __device__ inline int gx_head_max_width(const GxHeadDev& hd) { int s = 0; for (int j = 0; j < hd.k; ++j) s = hd.w[j] > s ? hd.w[j] : s; return s; }
+
 struct GxHparamsDev {
   int32_t iters;     // forward/backward/update iterations executed: num_epochs - 1 (the last epoch's backward is unobservable), num_epochs when a trace is requested
   int32_t out_iter;  // the mask (and the optimiser state) is emitted after this many updates: num_epochs - 1
@@ -383,7 +404,8 @@ cudaError_t gx_launch_explain_gang(const GxExplainLaunch& cfg, const GxGraphDev&
                                    const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                    float* out_mask, float* out_feat, cudaStream_t s);
 int gx_gang_smem_bytes(int d, int hid, int C);
-cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, float* H, float* pred, float* emb_out, float* P, cudaStream_t s);
+cudaError_t gx_launch_model_forward(const GxGraphDev& g, const GxModelDev& m, const GxHeadDev& hd, float* H, float* pred, float* emb_out, float* P,
+                                    cudaStream_t s);
 constexpr int GX_STREAM_THREADS = 768;  // 24 warps: 80 registers per thread, 5 KB of cp.async staging per warp
 int gx_explain_max_smem();
 struct GxGraphBatchDev {
@@ -399,12 +421,12 @@ cudaError_t gx_launch_explain_graphs(const GxExplainLaunch& cfg, const GxGraphBa
                                      float* out_feat, cudaStream_t s);
 // explain_var.cu: the model and optimiser variants, node mode (graph_mode 0, g) or graph mode (gb)
 cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
-                                  const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
+                                  const GxModelDev& m, const GxHeadDev& hd, const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,
                                   float* out_mask, float* out_feat, cudaStream_t s);
-int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C, int att = 0);
+int gx_var_smem_bytes(int graph_mode, int d, int L, int hid, int emb, int C, int att = 0, const GxHeadDev& hd = GxHeadDev{});
 constexpr int GX_VAR_WIDE_MIN = 129;    // input widths from here on run the variant kernel's wide path (layer 1 contracted as A_m (X B))
 constexpr int GX_VAR_WIDE_MAX = 4096;   // the largest input width the wide path builds
-int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m);
+int gx_var_ctas_per_sm(int graph_mode, const GxModelDev& m, const GxHeadDev& hd);
 int gx_var_row_stride(int hid, int emb);
 // explain_dense.cu: Explainer.explain(..., unconstrained=True), node mode (graph_mode 0, g) or graph mode (gb); m0 / out_dense are dense
 // (dense_off[t] = the offset of task t's n_t^2 block), out_mask holds the sub-adjacency slots, x.trace / x.trace_pred optional.
@@ -418,10 +440,10 @@ struct GxDenseIo {
   int32_t epochs;
 };
 cudaError_t gx_launch_explain_dense(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
-                                    const GxModelDev& m, const GxHparamsDev& hp, const GxPlanArrays& plan, const GxDenseIo& io,
-                                    cudaStream_t s);
-int gx_dense_smem_bytes(int d, int L, int hid, int emb, int C);
-int gx_dense_ctas_per_sm(const GxModelDev& m);
+                                    const GxModelDev& m, const GxHeadDev& hd, const GxHparamsDev& hp, const GxPlanArrays& plan,
+                                    const GxDenseIo& io, cudaStream_t s);
+int gx_dense_smem_bytes(int d, int L, int hid, int emb, int C, const GxHeadDev& hd = GxHeadDev{});
+int gx_dense_ctas_per_sm(const GxModelDev& m, const GxHeadDev& hd);
 cudaError_t gx_launch_outer_pairs(const GxHparamsDev& hp, const GxGraphDev& g, const GxPlanArrays& plan, int count,
                                   const float* m0, float* out_mask, const GxExtra& x, cudaStream_t s);
 cudaError_t gx_launch_denoise_topk(const GxPlanArrays& plan, int count, const float* edge_mask, int k2, int cap, float* out_thr,

@@ -86,6 +86,7 @@ struct gx_handle {
   // model
   bool has_model = false;
   GxModelDev m{};
+  GxHeadDev head{};   // the MLP prediction head of a gx_set_model_head model (k = 0: none); its block lies in m_buf
   DevBuf m_buf;
   // plan (node mode, or graph mode: one task per graph)
   bool has_plan = false;

@@ -419,7 +419,7 @@ static int explain_nodes_impl(gx_handle* h, const gx_hparams* hp, int mode, gx_m
       switch (kernel[c]) {
         case NodeKernel::smem:
         case NodeKernel::cluster: return gx_launch_explain(k, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
-        case NodeKernel::variant: return gx_launch_explain_var(k, 0, h->g, h->gb, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
+        case NodeKernel::variant: return gx_launch_explain_var(k, 0, h->g, h->gb, h->m, h->head, hd, h->plan, D.m0, D.out, D.feat, s);
         case NodeKernel::stream1: return gx_launch_explain_stream(k, h->g, h->m, hd, h->plan, D.m0, D.out, D.feat, s);
         case NodeKernel::gang: {
           const cudaError_t e = cudaMemsetAsync(k.gang_bars, 0, (size_t)(k.grid / k.gang) * 16, s);

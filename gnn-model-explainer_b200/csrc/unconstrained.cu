@@ -39,10 +39,10 @@ static int explain_unconstrained_impl(gx_handle* h, bool graph, const gx_hparams
     if (n > GX_DENSE_MAX_N) { gx_set_error("%s: task %d has n = %d > %d (the dense mask has n^2 parameters)", who, t, n, GX_DENSE_MAX_N); return GX_ERR_UNSUPPORTED; }
     doff[t + 1] = doff[t] + (int64_t)n * n;
   }
-  const int bytes = gx_dense_smem_bytes(h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C);
+  const int bytes = gx_dense_smem_bytes(h->m.d, h->m.L, h->m.hid, h->m.emb, h->m.C, h->head);
   if (bytes > gx_explain_max_smem()) { gx_set_error("%s: model does not fit the unconstrained kernel (%d bytes of shared memory)", who, bytes); return GX_ERR_UNSUPPORTED; }
   GX_CUDA_CHECK(cudaSetDevice(h->device));
-  const int per_sm = gx_dense_ctas_per_sm(h->m);
+  const int per_sm = gx_dense_ctas_per_sm(h->m, h->head);
   if (per_sm < 1) { gx_set_error("%s: the unconstrained kernel cannot be resident (%d bytes of shared memory)", who, bytes); return GX_ERR_UNSUPPORTED; }
   const int64_t dense = doff[count], te = h->total_e;
   GX_CUDA_CHECK(h->d_dense_off.reserve((size_t)(count + 1) * 8));
@@ -82,7 +82,7 @@ static int explain_unconstrained_impl(gx_handle* h, bool graph, const gx_hparams
     return gx_make_dense_layout(graph ? h->gb.max_nodes : T.n, h->m.d, h->m.L, vw).total_words; }, h->num_sms * per_sm, &cfg);
   if (rc == GX_OK) rc = begin_timing(h);
   if (rc != GX_OK) return rc;
-  GX_CUDA_CHECK(gx_launch_explain_dense(cfg, graph ? 1 : 0, h->g, h->gb, h->m, hd, h->plan, io, h->stream));
+  GX_CUDA_CHECK(gx_launch_explain_dense(cfg, graph ? 1 : 0, h->g, h->gb, h->m, h->head, hd, h->plan, io, h->stream));
   h->launches += 1;
   GX_CUDA_CHECK(cudaEventRecord(h->ev_t1, h->stream));
   h->timed = true;

@@ -15,6 +15,7 @@ GX_TRACE_COLS = 8
 TR_LOSS_EDGES, TR_PRED, TR_SIZE, TR_ENT, TR_LAP, TR_FEAT, TR_DENSITY, TR_PGT = range(8)
 GX_MODEL_BN = 1
 GX_MODEL_ATT = 2
+GX_MAX_HEAD_LAYERS = 4
 
 EXPORTS = [
     "gx_default_hparams", "gx_last_error", "gx_version", "gx_create", "gx_destroy", "gx_set_stream",
@@ -25,7 +26,7 @@ EXPORTS = [
     "gx_debug_force_stream", "gx_debug_ieee_edge", "gx_debug_set_dump", "gx_debug_set_gang", "gx_debug_set_cluster", "gx_denoise_topk",
     "gx_model_forward", "gx_comm_unique_id", "gx_comm_init", "gx_comm_destroy", "gx_count_nodes", "gx_allgather_masks", "gx_unshard_masks",
     "gx_plan_class_counts", "gx_last_class_ms", "gx_explain_nodes_unconstrained", "gx_explain_graphs_unconstrained",
-    "gx_set_model_att",
+    "gx_set_model_att", "gx_set_model_head",
 ]
 
 
@@ -83,6 +84,8 @@ def lib():
     L.gx_sync.argtypes = [vp]
     L.gx_set_model.argtypes = [vp, C.POINTER(GxModelDims), C.POINTER(vp), C.POINTER(vp), f32p, f32p]
     L.gx_set_model_att.argtypes = [vp, C.POINTER(GxModelDims), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), f32p, f32p]
+    L.gx_set_model_head.argtypes = [vp, C.POINTER(GxModelDims), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.c_int32, i32p, C.POINTER(vp),
+                                    C.POINTER(vp)]
     L.gx_set_graph_csr.argtypes = [vp, C.c_int64, i32p, i32p, f32p, C.c_int32, i32p, i32p]
     L.gx_neighborhood_rows.argtypes = [vp, i32p, C.c_int32, C.c_int32, vp]
     L.gx_plan_nodes.argtypes = [vp, i32p, C.c_int32, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]

@@ -103,10 +103,12 @@ class Engine:
     def sync(self):
         _abi.check(self._lib.gx_sync(self._h))
 
-    def set_model(self, weights, num_layers=3, bn=False, att=None):
+    def set_model(self, weights, num_layers=3, bn=False, att=None, head=None):
         """weights: dict W1,b1,W2,b2,W3,b3,Wp,bp (numpy; b* may be None).  Shapes are checked here: the C ABI takes bare
-        pointers, so a checkpoint whose layers do not chain (or a concat=False / MLP prediction head) must not reach it.
-        att: an attention model's (in, in) conv_*.att_weight matrices, one per layer (gx_set_model_att); None for any other model."""
+        pointers, so a checkpoint whose layers do not chain (or a concat=False model) must not reach it.
+        att: an attention model's (in, in) conv_*.att_weight matrices, one per layer (gx_set_model_att); None for any other model.
+        head: an MLP prediction head (pred_hidden_dims, models.py:193-207): [(W, b), ..] of its hidden Linears in order, torch's
+        (out, in) layout; Wp / bp are then its last Linear (C, last hidden width) (gx_set_model_head).  None: pred_model is one Linear."""
         Ws = [_f32c(weights["W%d" % (l + 1)]) for l in range(num_layers)]
         bs = [None if weights.get("b%d" % (l + 1)) is None else _f32c(weights["b%d" % (l + 1)])
               for l in range(num_layers)]
@@ -123,6 +125,18 @@ class Engine:
             if bs[l] is not None and bs[l].shape != (Ws[l].shape[1],):
                 raise ValueError("layer %d bias is %s, expected (%d,)" % (l + 1, bs[l].shape, Ws[l].shape[1]))
         pd = sum(w.shape[1] for w in Ws)
+        hw, hb = [], []
+        if head is not None:
+            if not 1 <= len(head) <= _abi.GX_MAX_HEAD_LAYERS:
+                raise NotImplementedError("an MLP prediction head of %d hidden layers is not built (1 .. %d)" % (len(head), _abi.GX_MAX_HEAD_LAYERS))
+            width = pd
+            for j, (w, b) in enumerate(head):
+                w, b = _f32c(w), _f32c(b)
+                if w.ndim != 2 or w.shape[1] != width or b.shape != (w.shape[0],):
+                    raise ValueError("head layer %d is %s / %s, expected (out, %d) / (out,)" % (j, w.shape, b.shape, width))
+                hw.append(w); hb.append(b)
+                width = w.shape[0]
+            pd = width      # the last Linear reads the last hidden layer
         if Wp.shape[1] != pd:
             if Wp.shape[1] == Ws[-1].shape[1]:
                 raise NotImplementedError("concat=False models (pred_model over the last layer only, models.py:113-116) are not built")
@@ -131,7 +145,20 @@ class Engine:
             raise ValueError("pred_model.bias is %s, expected (%d,)" % (bp.shape, Wp.shape[0]))
         wp = (C.c_void_p * num_layers)(*[w.ctypes.data for w in Ws])
         bp_arr = (C.c_void_p * num_layers)(*[(b.ctypes.data if b is not None else None) for b in bs])
-        if att is None:
+        if head is not None:
+            Was = [_f32c(a) for a in att] if att is not None else []
+            if att is not None and [a.shape for a in Was] != [(w.shape[0], w.shape[0]) for w in Ws]:
+                raise ValueError("att_weight shapes %s do not match the conv layers" % [a.shape for a in Was])
+            dims = _abi.GxModelDims(Ws[0].shape[0], Ws[0].shape[1], Ws[-1].shape[1], Wp.shape[0], num_layers,
+                                    (_abi.GX_MODEL_BN if bn else 0) | (_abi.GX_MODEL_ATT if att is not None else 0))
+            ap = (C.c_void_p * num_layers)(*[a.ctypes.data for a in Was]) if att is not None else None
+            widths = np.asarray([w.shape[0] for w in hw], np.int32)
+            lw = hw + [Wp]
+            lb = hb + [bp]
+            hwp = (C.c_void_p * len(lw))(*[w.ctypes.data for w in lw])
+            hbp = (C.c_void_p * len(lb))(*[b.ctypes.data for b in lb])
+            _abi.check(self._lib.gx_set_model_head(self._h, C.byref(dims), wp, bp_arr, ap, len(hw), _np_ptr(widths), hwp, hbp))
+        elif att is None:
             dims = _abi.GxModelDims(Ws[0].shape[0], Ws[0].shape[1], Ws[-1].shape[1], Wp.shape[0], num_layers,
                                     _abi.GX_MODEL_BN if bn else 0)
             _abi.check(self._lib.gx_set_model(self._h, C.byref(dims), wp, bp_arr, _np_ptr(Wp), _np_ptr(bp)))

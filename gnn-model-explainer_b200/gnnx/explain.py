@@ -52,10 +52,19 @@ def gen_explainer_prefix(args):
 def model_weights(model):
     """state_dict of a reference (or gnnx) GcnEncoderNode/GcnEncoderGraph -> weight dict.
     Keys as in the reference checkpoints (SURVEY 8a8): conv_first / conv_block.i / conv_last /
-    pred_model; an attention model (--method att) also has <layer>.att_weight, returned as Wa1 .. WaL."""
+    pred_model; an attention model (--method att) also has <layer>.att_weight, returned as Wa1 .. WaL.  A model with an MLP
+    prediction head (pred_hidden_dims, models.py:193-207: pred_model.0 / .2 / .. Linears around ReLUs) returns its hidden Linears as
+    "head" = [(W, b), ..] (torch's (out, in) layout) and its last Linear as Wp / bp."""
     sd = {k: v.detach().cpu().float().numpy() for k, v in model.state_dict().items()}
+    head = []
     if "pred_model.weight" not in sd:
-        raise NotImplementedError("pred_hidden_dims != [] (MLP prediction head) is not built")
+        j = 0
+        while ("pred_model.%d.weight" % j) in sd:
+            head.append((sd["pred_model.%d.weight" % j], sd["pred_model.%d.bias" % j]))
+            j += 2
+        if len(head) < 2 or any(k.startswith("pred_model.") and not k.startswith(tuple("pred_model.%d." % i for i in range(0, j, 2)))
+                                for k in sd):
+            raise ValueError("pred_model is neither a Linear nor the Sequential(Linear, ReLU, .., Linear) of pred_hidden_dims")
     n_block = 0
     while ("conv_block.%d.weight" % n_block) in sd:
         n_block += 1
@@ -70,7 +79,10 @@ def model_weights(model):
             w["Wa%d" % l] = sd[nm + ".att_weight"]
     if any(("Wa%d" % l) in w for l in range(1, len(names) + 1)) and not all(("Wa%d" % l) in w for l in range(1, len(names) + 1)):
         raise ValueError("att_weight on some conv layers only")
-    w["Wp"], w["bp"] = sd["pred_model.weight"], sd["pred_model.bias"]
+    if head:
+        (w["Wp"], w["bp"]), w["head"] = head[-1], head[:-1]
+    else:
+        w["Wp"], w["bp"] = sd["pred_model.weight"], sd["pred_model.bias"]
     return w, len(names)
 
 
@@ -107,8 +119,10 @@ class Explainer:
         weights, num_layers = model_weights(model)
         self._att = "Wa1" in weights
         self._wide = weights["W1"].shape[0] > 128   # inputs wider than 128: the variant kernel's wide path
+        self._head = "head" in weights             # an MLP prediction head (pred_hidden_dims): the variant kernel
         self.engine.set_model(weights, num_layers=num_layers, bn=bn,
-                              att=[weights["Wa%d" % l] for l in range(1, num_layers + 1)] if self._att else None)
+                              att=[weights["Wa%d" % l] for l in range(1, num_layers + 1)] if self._att else None,
+                              head=weights.get("head"))
         if getattr(args, "gnnx_latency", False):
             self.engine.debug_cluster(0, 0)   # latency mode: thread-block clusters for the expensive tasks of batches that leave SMs idle
         # model / optimiser variants run in the variant kernel, which does not log the per-epoch trace print_training replays: the
@@ -117,7 +131,7 @@ class Explainer:
         self._max_width = max(weights["W%d" % l].shape[1] for l in range(1, num_layers + 1))
         self._wide_layers = self._max_width > 32
         self._no_trace = (bn or num_layers != 3 or self._wide_layers or getattr(args, "opt", "adam") != "adam" or self._att
-                          or self._wide)
+                          or self._wide or self._head)
         adj_np = np.asarray(adj)
         if graph_mode:
             # graph classification: the whole padded batch goes to the device once (explain.py:80-85)
@@ -247,6 +261,8 @@ class Explainer:
         plan = self.engine.plan_nodes(nodes, self.n_hops)
         edge_mask = np.empty(plan.total_edges, dtype=np.float32)
         if model == "grad":        # explain.py:125-133: one backward to the adjacency, no mask parameters
+            if self._head:
+                raise NotImplementedError("model='grad' is not built for models with an MLP prediction head (pred_hidden_dims)")
             try:
                 self.engine.grad_nodes_host(edge_mask)     # (unconstrained is ignored here, as in the reference)
             except _abi.GnnxError as e:
@@ -293,7 +309,9 @@ class Explainer:
             raise NotImplementedError("unconstrained=True is not built for hidden / output widths above 128 (this model: %d)" % self._max_width)
 
     def _print_no_trace(self):
-        if self._att:
+        if self._head:
+            print("(per-epoch trace is not built for models with an MLP prediction head (pred_hidden_dims))")
+        elif self._att:
             print("(per-epoch trace is not built for attention models (--method att))")
         elif self._wide:
             print("(per-epoch trace is not built for inputs wider than 128 features)")

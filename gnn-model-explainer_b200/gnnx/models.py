@@ -55,8 +55,6 @@ class GcnEncoderGraph(nn.Module):
     def __init__(self, input_dim, hidden_dim, embedding_dim, label_dim, num_layers, pred_hidden_dims=[],
                  concat=True, bn=True, dropout=0.0, add_self=False, args=None):
         super().__init__()
-        if len(pred_hidden_dims) != 0:
-            raise NotImplementedError("pred_hidden_dims != [] is not built")
         self.concat = concat
         self.bn = bn
         self.num_layers = num_layers
@@ -71,7 +69,7 @@ class GcnEncoderGraph(nn.Module):
         self.act = nn.ReLU()
         self.label_dim = label_dim
         self.pred_input_dim = hidden_dim * (num_layers - 1) + embedding_dim if concat else embedding_dim
-        self.pred_model = nn.Linear(self.pred_input_dim, label_dim)
+        self.pred_model = self.build_pred_layers(self.pred_input_dim, pred_hidden_dims, label_dim)
         for m in self.modules():
             if isinstance(m, GraphConv):
                 init.xavier_uniform_(m.weight.data, gain=nn.init.calculate_gain("relu"))
@@ -79,6 +77,19 @@ class GcnEncoderGraph(nn.Module):
                     init.xavier_uniform_(m.att_weight.data, gain=nn.init.calculate_gain("relu"))
                 if m.bias is not None:
                     init.constant_(m.bias.data, 0.0)
+
+    def build_pred_layers(self, in_width, hidden_widths, num_classes):
+        """pred_model (models.py:193-207): a single Linear(in_width, num_classes) without hidden widths; otherwise an nn.Sequential that
+        alternates Linear and the shared ReLU module and ends in a Linear to num_classes, so that the Linears sit at the even indices
+        (state_dict keys pred_model.0 / .2 / ..).  Every Linear has a bias and torch's default init, drawn in the order the layers are
+        listed, which is the reference's order of draws."""
+        if not hidden_widths:
+            return nn.Linear(in_width, num_classes)
+        widths = [in_width] + list(hidden_widths)
+        mods = []
+        for w_in, w_out in zip(widths[:-1], widths[1:]):
+            mods += [nn.Linear(w_in, w_out), self.act]
+        return nn.Sequential(*mods, nn.Linear(widths[-1], num_classes))
 
     def apply_bn(self, x):
         bn_module = nn.BatchNorm1d(x.size()[1]).to(x.device)

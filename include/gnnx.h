@@ -154,6 +154,18 @@ int gx_set_model(gx_handle* h, const gx_model_dims* dims, const float* const* co
 int gx_set_model_att(gx_handle* h, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
                      const float* const* att_w, const float* pred_w, const float* pred_b);
 
+/* Model with an MLP prediction head (GcnEncoderNode / GcnEncoderGraph(pred_hidden_dims=[h1 .. hk]), models.py:193-207): pred_model
+ * is Sequential(Linear(PD, h1), ReLU, .., Linear(hk, C)) over the concatenated embedding, PD = hidden_dim (num_layers - 1) +
+ * embed_dim.  gx_set_model's arguments (att_w: as gx_set_model_att for an attention model, NULL for any other) plus head_layers = k,
+ * head_widths[k], and head_w / head_b: k + 1 pointers to the Linear weights, row-major (out, in) as in the state_dict
+ * (pred_model.0.weight, pred_model.2.weight, ..), and their biases (never NULL: every Linear has one).  Runs on the model-variant
+ * kernel (mask optimisation only: no trace, optimiser state, GX_INIT_STATE or grad).  GX_ERR_UNSUPPORTED beyond
+ * GX_MAX_HEAD_LAYERS hidden layers or GX_MAX_WIDTH per head width. */
+#define GX_MAX_HEAD_LAYERS 4
+int gx_set_model_head(gx_handle* h, const gx_model_dims* dims, const float* const* conv_w, const float* const* conv_b,
+                      const float* const* att_w, int32_t head_layers, const int32_t* head_widths, const float* const* head_w,
+                      const float* const* head_b);
+
 /* Graph of a node-classification task, replacing Explainer(adj, feat, label, pred) (explain.py:43-62):
  * CSR of the (B=1) adjacency with ascending columns per row (must be symmetric 0/1; self loops are
  * honoured by gx_plan_nodes' reachability and dropped from the explained edge set exactly like the
