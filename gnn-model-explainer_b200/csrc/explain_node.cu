@@ -155,6 +155,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
   __shared__ GxLayout sL;
   __shared__ int s_long[3];  // number of long rows among [0,n2), among [0,n1), and rows with a long < n1 prefix
   static_assert(HID % 4 == 0 && EMB % 4 == 0, "hidden widths must be multiples of 4");
+  static_assert(sizeof(IdxT) == 2, "the pair slab packs two indices per word");
   constexpr IdxT kNone = IdxTraits<IdxT>::kNone;
   constexpr int HS = HID;            // row stride of the hidden-width arrays
   constexpr int H4 = HID / 4;
@@ -187,7 +188,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
     // gradient baseline: the loss is taken at the node's PREDICTED label (explain.py:130), otherwise at label[node] (explain.py:750-753)
     const int gt = hp.mode ? __ldg(A.g.pred_label + Tp->node) : Tp->gt_label;
     const int64_t node_off = Tp->node_off, rp_off = Tp->rp_off, edge_off = Tp->edge_off, pair_off = Tp->pair_off;
-    if (tid == 0) sL = gx_make_layout(n, n1, n2, e1, np, d, HID, EMB, C, nwarps, (int)sizeof(IdxT), CS);
+    if (tid == 0) sL = gx_make_layout(n, n1, n2, e1, d, HID, EMB, C, nwarps, (int)sizeof(IdxT), CS);
     __syncthreads();
     const int dp = sL.dp, D4 = dp / 4;
     const int32_t* __restrict__ lo2gid = A.plan.lo2gid + node_off;
@@ -201,9 +202,8 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
       float* const bs = base + sL.bs; float* const sF = base + sL.sF; float* const Fm = base + sL.F; float* const mF = base + sL.mF;
       float* const vF = base + sL.vF; float* const gFp = base + sL.gFp; float* const a = base + sL.a; float* const yv = base + sL.y;
       float2* const MM = reinterpret_cast<float2*>(A.pws + (int64_t)cid * A.pws_stride_words); float2* const mm = MM + np; float2* const vv = mm + np; float2* const SS = vv + np;
+      uint2* const PX = reinterpret_cast<uint2*>(SS + np);
       IdxT* const icol = reinterpret_cast<IdxT*>(base + sL.icol); IdxT* const irp = reinterpret_cast<IdxT*>(base + sL.irp);
-      IdxT* const pi = reinterpret_cast<IdxT*>(base + sL.pi); IdxT* const pj = reinterpret_cast<IdxT*>(base + sL.pj);
-      IdxT* const ppij = reinterpret_cast<IdxT*>(base + sL.ppij); IdxT* const ppji = reinterpret_cast<IdxT*>(base + sL.ppji);
     for (int idx = tid; idx < n * dp; idx += nthreads) {
       const int i = idx / dp, f = idx - i * dp;
       X[idx] = f < d ? __ldg(A.g.feat + (int64_t)lo2gid[i] * d + f) : 0.f;
@@ -255,9 +255,6 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
       const int i = A.plan.pair_i[pair_off + p], j = A.plan.pair_j[pair_off + p];
       const int pij = A.plan.pair_pij[pair_off + p], pji = A.plan.pair_pji[pair_off + p];
       const int oij = A.plan.pair_oij[pair_off + p], oji = A.plan.pair_oji[pair_off + p];
-      pi[p] = (IdxT)i; pj[p] = (IdxT)j;
-      ppij[p] = i < n2 ? (IdxT)pij : kNone;
-      ppji[p] = j < n2 ? (IdxT)pji : kNone;
       float Mi, Mj;
       if (hp.mode) {
         Mi = Mj = 0.f;
@@ -280,6 +277,9 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         mm[p] = m2;
         vv[p] = v2;
         SS[p] = make_float2(Si, Sj);
+        // (i, j) and the pair's slots in rows i and j of `a` (kNone: the row is beyond n2), two 16-bit indices per word
+        PX[p] = make_uint2((uint32_t)i | ((uint32_t)j << 16),
+                           (uint32_t)(i < n2 ? (IdxT)pij : kNone) | ((uint32_t)(j < n2 ? (IdxT)pji : kNone) << 16));
       }
       const float a0 = hp.mode ? 1.0f : 0.5f * (Si + Sj);  // explain.py:665-678 ; gradient baseline: the adjacency itself
       if (i < n2) a[pij] = a0;
@@ -552,8 +552,6 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         float* const gFp = base + sL.gFp;
         float* const sF = base + sL.sF;
         float* const Fm = base + sL.F; float* const mF = base + sL.mF; float* const vF = base + sL.vF;
-        const IdxT* const pi = reinterpret_cast<const IdxT*>(base + sL.pi); const IdxT* const pj = reinterpret_cast<const IdxT*>(base + sL.pj);
-        const IdxT* const ppij = reinterpret_cast<const IdxT*>(base + sL.ppij); const IdxT* const ppji = reinterpret_cast<const IdxT*>(base + sL.ppji);
         const float* const yv = base + sL.y;
         const float* const dZ1s = base + sL.U;
         float* const X = base + sL.X;
@@ -562,7 +560,11 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         float* const dZ3 = base + sL.dZ3;
         float* const Yh2 = base + sL.Yh2;
         float2* const MM = reinterpret_cast<float2*>(A.pws + (int64_t)cid * A.pws_stride_words); float2* const mm = MM + np; float2* const vv = mm + np; float2* const SS = vv + np;
+        const uint2* const PX = reinterpret_cast<const uint2*>(SS + np);
         float* const a = base + sL.a;
+        // the pairs' indices come from the L2-resident slab one round ahead of their use: the dots below wait for no L2 round trip
+        const int p0 = cwarp * 32 + lane, pstride = nthreads * CS;
+        uint2 pxn = p0 < np ? PX[p0] : make_uint2(0u, 0u);
         const float2 tab = __ldg(hp.adam_tab + (it - 1));
         const float step = tab.x, bc2s = tab.y, bc2s_inv = 1.0f / tab.y;
         const bool last = (it == hp.out_iter);   // the mask built after this update is the one the reference returns
@@ -593,8 +595,10 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         float trS = 0.f, trH = 0.f, trL = 0.f, trD = 0.f;   // trace: this thread's share of sum S, sum H(S), sum a (y_i-y_j)^2, sum 2a'
         if (hp.mode) {
           // gradient baseline (explain.py:125-133): mask_ij = sigmoid(|dL/dA_ij| + |dL/dA_ji|) on the edges, no regulariser, no update
-          for (int p = cwarp * 32 + lane; p < np; p += nthreads * CS) {
-            const int i = pi[p], j = pj[p];
+          for (int p = p0; p < np; p += pstride) {
+            const uint2 px = pxn;
+            if (p + pstride < np) pxn = PX[p + pstride];
+            const int i = px.x & 0xffffu, j = px.x >> 16;
             float gij = 0.f, gji = 0.f;
             if (i < n2) gij += dot_v4(dZ1s + i * dp, X + j * dp, D4);
             if (j < n2) gji += dot_v4(dZ1s + j * dp, X + i * dp, D4);
@@ -606,12 +610,14 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
             A.out_mask[edge_off + A.plan.pair_oji[pair_off + p]] = an;
           }
         } else
-        for (int p = cwarp * 32 + lane; p < np; p += nthreads * CS) {
+        for (int p = p0; p < np; p += pstride) {
           // optimiser state of the pair (L2-resident slab): issued first so that the L2 round trip overlaps the dots below
           float2 Mv = MM[p];
           const float2 Sv = SS[p];
           float2 m2 = mm[p], v2 = vv[p];
-          const int i = pi[p], j = pj[p];
+          const uint2 px = pxn;
+          if (p + pstride < np) pxn = PX[p + pstride];
+          const int i = px.x & 0xffffu, j = px.x >> 16;
           const float yd = yv[i] - yv[j];
           float Gd = lap_over_nn * yd * yd;  // d/dA_ij + d/dA_ji of y^T (D - A) y / n^2 (explain.py:780-793)
           if (kTrace) {
@@ -637,7 +643,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
           MM[p] = Mv; mm[p] = m2; vv[p] = v2; SS[p] = Sn;
           const float an = 0.5f * (Sn.x + Sn.y);
           if (kTrace) trD += 2.0f * an;
-          const IdxT pa = ppij[p], pb = ppji[p];
+          const IdxT pa = (IdxT)(px.y & 0xffffu), pb = (IdxT)(px.y >> 16);
           if (pa != kNone) peer.st1(a + pa, an);
           if (pb != kNone) peer.st1(a + pb, an);
           if (last) {

@@ -140,16 +140,17 @@ struct GxLayout {
   // float arrays (offsets in 4-byte words)
   int X, U, Yh1, q1, Yh2, q2, dZ2, a, y, W1s, W1t, W2s, W2t, W3s, bs, sF, F, mF, vF, gFp, zs, dE, dZ3, logit, Wp;
   // index arrays (offsets in 4-byte words; element type IdxT)
-  int icol, irp, pi, pj, ppij, ppji, llist, cnt1, llistB;
+  int icol, irp, llist, cnt1, llistB;
   int total_words;
   int dp;
 };
 
-// Shared-memory footprint of one task.  np_in = pairs with an endpoint in rows < n2 (their indices live in
-// shared memory, their optimiser state in a per-CTA global slab that stays in L2); pairs between two
-// outermost nodes never touch the forward and are optimised by a separate elementwise kernel.
+// Shared-memory footprint of one task.  np_in = pairs with an endpoint in rows < n2: their optimiser state and
+// their indices live in a per-CTA global slab that stays in L2 (read once per epoch, in the pair phase, so
+// shared memory would only buy latency the phase already hides); pairs between two outermost nodes never
+// touch the forward and are optimised by a separate elementwise kernel.
 // idx_bytes = sizeof(IdxT) (2 or 4).  hid/emb must be multiples of 4.
-__host__ __device__ inline GxLayout gx_make_layout(int n, int n1, int n2, int e1, int np_in, int d,
+__host__ __device__ inline GxLayout gx_make_layout(int n, int n1, int n2, int e1, int d,
                                                    int hid, int emb, int C, int nwarps,
                                                    int idx_bytes, int cs = 1) {
   GxLayout L;
@@ -185,10 +186,6 @@ __host__ __device__ inline GxLayout gx_make_layout(int n, int n1, int n2, int e1
   L.Wp = takef(C * (2 * hid + emb + 1) <= GX_WP_SMEM_MAX ? C * (2 * hid + emb + 1) : 0);  // pred_model weights + bias when small
   L.icol = takei(e1);
   L.irp = takei(n2 + 1);
-  L.pi = takei(np_in);
-  L.pj = takei(np_in);
-  L.ppij = takei(np_in);
-  L.ppji = takei(np_in);
   L.llist = takei(n2);
   L.cnt1 = takei(n2);        // per row: number of leading columns < n1 (the only ones that carry dZ2)
   L.llistB = takei(n2);      // rows whose < n1 prefix is long (split across a whole warp in the backward)

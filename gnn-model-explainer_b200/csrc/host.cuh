@@ -67,7 +67,7 @@ struct gx_handle {
   float* dbg = nullptr;
   // knobs, read from the environment by gx_create; the gx_debug_* entry points set the test knobs later
   LaunchClass classes[kNumClasses];   // kNodeClasses with GNNX_CLASS_THREADS applied
-  int exclusive_topk = 12;    // GNNX_EXCLUSIVE_TOPK: tasks of the 2-per-SM class that may get an SM of their own
+  int exclusive_topk = 30;    // GNNX_EXCLUSIVE_TOPK: tasks of the 2-per-SM class that may get an SM of their own (syn1 sweep, DESIGN section 6)
   bool host_timing = false;   // GNNX_HOST_TIMING=1: stderr breakdown of the host side (tools/)
   bool ieee_edge = false;     // test knob (gx_debug_ieee_edge / GNNX_IEEE_EDGE): IEEE arithmetic in the edge phase
   int gang_override = 0;      // test knob (gx_debug_set_gang / GNNX_GANG): CTAs per task of explain_gang.cu, 0 = automatic, -1 = explain_stream.cu
@@ -176,9 +176,10 @@ void fill_hparams(const gx_handle* h, const gx_hparams* hp, int mode, bool trace
 int upload_dense_offsets(gx_handle* h, int64_t* total);
 int begin_timing(gx_handle* h);
 
-// Pair-state slab of one CTA: 8 floats per inner pair (all pairs in graph mode) of the largest task it may take.  Slabs are per CTA and
-// the work queue is dynamic, so the stride never changes a result.
-inline int64_t pair_slab_words(int max_pairs) { return ((int64_t)max_pairs * 8 + 3) / 4 * 4; }
+// Pair-state slab of one CTA: 8 floats of optimiser state per inner pair (all pairs in graph mode) of the largest task it may take,
+// and 2 words for the pair's four 16-bit indices (explain_node.cu).  Slabs are per CTA and the work queue is dynamic, so the stride
+// never changes a result.
+inline int64_t pair_slab_words(int max_pairs) { return ((int64_t)max_pairs * 10 + 3) / 4 * 4; }
 
 // Places the pair slabs of n launches one after another in d_pws (launch c: slabs[c] slabs of cfg[c].pws_stride_words) and points
 // cfg[c].pws at them.

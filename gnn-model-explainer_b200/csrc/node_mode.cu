@@ -49,7 +49,7 @@ int task_smem_class(const gx_handle* h, const GxTask& T, int* bytes_out) {
   const bool small_idx = !h->force_stream && T.n < 65535 && T.e1 < 65535;
   for (int c = 0; small_idx && c < kStreamClass; ++c) {
     const int nwarps = h->classes[c].threads / 32;
-    const GxLayout L = gx_make_layout(T.n, T.n1, T.n2, T.e1, T.npairs_in, m.d, m.hid, m.emb, m.C, nwarps, 2);
+    const GxLayout L = gx_make_layout(T.n, T.n1, T.n2, T.e1, m.d, m.hid, m.emb, m.C, nwarps, 2);
     const int64_t bytes = (int64_t)L.total_words * 4;
     if (bytes <= h->classes[c].cap_bytes) {
       *bytes_out = (int)bytes;
@@ -199,7 +199,7 @@ int gx_plan_nodes(gx_handle* h, const int32_t* nodes, int32_t count, int32_t n_h
     int cls = h->m.variant ? kStreamClass : task_smem_class(h, T, &bytes);
     if (cls < kStreamClass && g_cluster_size > 1 && cost(t) > g_cluster_cost) {
       // expensive task: one thread-block cluster (explain_node.cu, CS CTAs share the rows and pairs); decided by the task alone
-      const GxLayout L = gx_make_layout(T.n, T.n1, T.n2, T.e1, T.npairs_in, h->m.d, h->m.hid, h->m.emb, h->m.C, cluster_cls.threads / 32, 2, g_cluster_size);
+      const GxLayout L = gx_make_layout(T.n, T.n1, T.n2, T.e1, h->m.d, h->m.hid, h->m.emb, h->m.C, cluster_cls.threads / 32, 2, g_cluster_size);
       if ((int64_t)L.total_words * 4 <= cluster_cls.cap_bytes) { cls = kClusterClass; bytes = L.total_words * 4; }
     }
     T.smem_bytes = bytes;
@@ -229,7 +229,7 @@ int gx_plan_nodes(gx_handle* h, const int32_t* nodes, int32_t count, int32_t n_h
         int k = 0;
         while (k < (int)cand.size() && (k + 1) * cs <= spare && lat(cand[k]) / cs + ovh < lat(cand[k])) {
           const GxTask& T = h->tasks[cand[k]];
-          const GxLayout L = gx_make_layout(T.n, T.n1, T.n2, T.e1, T.npairs_in, h->m.d, h->m.hid, h->m.emb, h->m.C, cluster_cls.threads / 32, 2, cs);
+          const GxLayout L = gx_make_layout(T.n, T.n1, T.n2, T.e1, h->m.d, h->m.hid, h->m.emb, h->m.C, cluster_cls.threads / 32, 2, cs);
           if ((int64_t)L.total_words * 4 > cluster_cls.cap_bytes) break;
           ++k;
         }
@@ -243,7 +243,7 @@ int gx_plan_nodes(gx_handle* h, const int32_t* nodes, int32_t count, int32_t n_h
       for (int i = 0; i < best_k; ++i) {
         const int32_t t = cand[i];
         GxTask& T = h->tasks[t];
-        const GxLayout L = gx_make_layout(T.n, T.n1, T.n2, T.e1, T.npairs_in, h->m.d, h->m.hid, h->m.emb, h->m.C, cluster_cls.threads / 32, 2, best_cs);
+        const GxLayout L = gx_make_layout(T.n, T.n1, T.n2, T.e1, h->m.d, h->m.hid, h->m.emb, h->m.C, cluster_cls.threads / 32, 2, best_cs);
         T.smem_bytes = L.total_words * 4;
         for (int c : {kTwoClass, kOneClass}) {
           auto& v = h->class_order[c];
