@@ -163,7 +163,7 @@ void fill_hparams(const gx_handle* h, const gx_hparams* hp, int mode, bool trace
   hd->c_size = hp->coef_size; hd->c_feat_size = hp->coef_feat_size; hd->c_ent = hp->coef_ent; hd->c_lap = hp->coef_lap;
   hd->adam_tab = h->d_adam.as<float2>();
   hd->init = hp->init;
-  hd->flags = h->ieee_edge ? GX_HP_IEEE_EDGE : 0;
+  hd->flags = (h->ieee_edge ? GX_HP_IEEE_EDGE : 0) | (h->node_generic ? GX_HP_NODE_GENERIC : 0);
   hd->mode = mode;
   hd->opt = hp->opt;
   hd->seed = hp->seed;
@@ -404,6 +404,7 @@ int gx_create(int device, gx_handle** out) {
   if (const char* env = getenv("GNNX_CLUSTER_SIZE")) { const int v = atoi(env); if (v == 0 || v == 1 || v == 2 || v == 4) h->cluster_size = v; }
   if (const char* env = getenv("GNNX_CLUSTER_COST")) { const long long v = atoll(env); if (v > 0) h->cluster_cost = v; }
   if (const char* env = getenv("GNNX_IEEE_EDGE")) h->ieee_edge = atoi(env) != 0;
+  if (const char* env = getenv("GNNX_NODE_GENERIC")) h->node_generic = atoi(env) != 0;
   for (int i = 0; i < kNumClasses; ++i) {
     GX_CUDA_CHECK(cudaStreamCreateWithFlags(&h->side[i], cudaStreamNonBlocking));
     GX_CUDA_CHECK(cudaEventCreate(&h->ev_join[i]));

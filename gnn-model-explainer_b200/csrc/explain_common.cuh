@@ -77,12 +77,20 @@ __device__ __forceinline__ void fma4(float4& acc, float s, const float4 v) {
   acc.x = fmaf(s, v.x, acc.x); acc.y = fmaf(s, v.y, acc.y); acc.z = fmaf(s, v.z, acc.z); acc.w = fmaf(s, v.w, acc.w);
 }
 
-// dot of two length-(4*n4) vectors / dot(a, relu(b))
+// dot of two length-(4*n4) vectors / dot(a, relu(b)).  kMaxN4 > 0: n4 <= kMaxN4, unrolled to that bound with k < n4 as a predicate
+template <int kMaxN4 = 0>
 __device__ __forceinline__ float dot_v4(const float* a, const float* b, int n4) {
   float s = 0.f;
-  for (int k = 0; k < n4; ++k) {
+  const auto step = [&](int k) {
     const float4 x = ld4(a + 4 * k), y = ld4(b + 4 * k);
     s = fmaf(x.x, y.x, s); s = fmaf(x.y, y.y, s); s = fmaf(x.z, y.z, s); s = fmaf(x.w, y.w, s);
+  };
+  if constexpr (kMaxN4 > 0) {
+#pragma unroll
+    for (int k = 0; k < kMaxN4; ++k)
+      if (k < n4) step(k);
+  } else {
+    for (int k = 0; k < n4; ++k) step(k);
   }
   return s;
 }
@@ -181,22 +189,41 @@ struct Grp {
   int GW, epi, grp, q, gbase, lane;
 };
 
-// sum of v over the GW lanes of the caller's group (every lane of the warp must call this)
+// sum of v over the GW lanes of the caller's group (every lane of the warp must call this).  kGW > 0: GW == kGW is known
+// at compile time, so the shuffles are issued together; the adds keep their left-to-right order either way.
+template <int kGW = 0>
 __device__ __forceinline__ float group_sum(float v, const Grp& G) {
   float s = 0.f;
-  for (int k = 0; k < G.GW; ++k) s += __shfl_sync(0xffffffffu, v, min(G.gbase + k, 31));
+  if constexpr (kGW > 0) {
+    float t[kGW];
+#pragma unroll
+    for (int k = 0; k < kGW; ++k) t[k] = __shfl_sync(0xffffffffu, v, min(G.gbase + k, 31));
+#pragma unroll
+    for (int k = 0; k < kGW; ++k) s += t[k];
+  } else {
+    for (int k = 0; k < G.GW; ++k) s += __shfl_sync(0xffffffffu, v, min(G.gbase + k, 31));
+  }
   return s;
 }
 
-// out4 = init + sum_{f < 4*F4} z[f] * W[f][4q .. 4q+3]   (z: F4 float4 in the group's scratch row)
+__device__ __forceinline__ void group_dense_step(const float* zrow, int f4, const float* W, int ldw, int q, float4& acc) {
+  const float4 z = ld4(zrow + 4 * f4);
+  const float* w = W + (4 * f4) * ldw + 4 * q;
+  fma4(acc, z.x, ld4(w));
+  fma4(acc, z.y, ld4(w + ldw));
+  fma4(acc, z.z, ld4(w + 2 * ldw));
+  fma4(acc, z.w, ld4(w + 3 * ldw));
+}
+// out4 = init + sum_{f < 4*F4} z[f] * W[f][4q .. 4q+3]   (z: F4 float4 in the group's scratch row).  kMaxF4 > 0: F4 <= kMaxF4,
+// and the loop is unrolled to that bound with f4 < F4 as a predicate.
+template <int kMaxF4 = 0>
 __device__ __forceinline__ float4 group_dense(const float* zrow, int F4, const float* W, int ldw, int q, float4 acc) {
-  for (int f4 = 0; f4 < F4; ++f4) {
-    const float4 z = ld4(zrow + 4 * f4);
-    const float* w = W + (4 * f4) * ldw + 4 * q;
-    fma4(acc, z.x, ld4(w));
-    fma4(acc, z.y, ld4(w + ldw));
-    fma4(acc, z.z, ld4(w + 2 * ldw));
-    fma4(acc, z.w, ld4(w + 3 * ldw));
+  if constexpr (kMaxF4 > 0) {
+#pragma unroll
+    for (int f4 = 0; f4 < kMaxF4; ++f4)
+      if (f4 < F4) group_dense_step(zrow, f4, W, ldw, q, acc);
+  } else {
+    for (int f4 = 0; f4 < F4; ++f4) group_dense_step(zrow, f4, W, ldw, q, acc);
   }
   return acc;
 }

@@ -147,19 +147,26 @@ __device__ __forceinline__ void readout_phase(int lane, int C, int gt, const Idx
 // CS > 1: cluster launch class -- the CS CTAs of a thread-block cluster share one task (rows and pairs dealt over the cluster's
 // warps, results stored into every CTA's copy of the state through DSMEM, hardware cluster barrier between phases; phases S and
 // B2 concern a handful of rows and are computed redundantly by every CTA, which saves two cluster barriers per epoch).
-template <typename IdxT, int HID, int EMB, int NT, bool kTrace, int CS>
+// kNarrow: 4*ceil(d/4) <= HID == EMB (every default-width model with d <= HID; checked by the launcher).  The lane group is then
+// GW = HID/4 lanes wide at compile time, and the loops over the input width run to the constant H4 with the run-time D4 as a
+// predicate: the same arithmetic in the same order as the run-time shape, with fewer instructions and registers.
+template <typename IdxT, int HID, int EMB, int NT, bool kTrace, int CS, bool kNarrow>
 __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const ExplainArgs A) {
   extern __shared__ __align__(16) float smem_dyn[];
   __shared__ int s_task;
   __shared__ float s_tr[kTrace ? (NT / 32) * CS * 4 + 4 : 1];   // trace: per-warp partial sums of the edge phase + (pred loss, p[gt], feat-size term)
   __shared__ GxLayout sL;
   __shared__ int s_long[3];  // number of long rows among [0,n2), among [0,n1), and rows with a long < n1 prefix
+  __shared__ long long s_clk[8];   // A.dbg only (thread 0): clock64 sums of the phases F1 F2 S B2 B1 P, the last mark, the task's start (globaltimer ns)
   static_assert(HID % 4 == 0 && EMB % 4 == 0, "hidden widths must be multiples of 4");
   static_assert(sizeof(IdxT) == 2, "the pair slab packs two indices per word");
+  static_assert(!kNarrow || (CS == 1 && EMB == HID), "the narrow instantiation is for single-CTA tasks of HID == EMB models");
   constexpr IdxT kNone = IdxTraits<IdxT>::kNone;
   constexpr int HS = HID;            // row stride of the hidden-width arrays
   constexpr int H4 = HID / 4;
   constexpr int PD = 2 * HID + EMB;  // pred_model input width (concat of the three layers)
+  constexpr int kF4 = kNarrow ? H4 : 0;   // compile-time bound of the loops over D4 (0: run-time trip count)
+  constexpr int kGW = kNarrow ? H4 : 0;   // compile-time lane-group width (0: run-time)
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nthreads = blockDim.x, nwarps = nthreads >> 5;
   const int crank = CS > 1 ? (int)cluster_ctarank() : 0;        // this CTA's rank in its cluster
@@ -181,8 +188,11 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
     phase_sync<CS>();
     if (qi >= A.ntasks) break;
     const int task_id = A.order[qi];
-    unsigned long long t_start_ns = 0;
-    if (A.dbg != nullptr && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start_ns));
+    if (A.dbg != nullptr && tid == 0) {
+      unsigned long long t_start_ns;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start_ns));
+      s_clk[7] = (long long)t_start_ns;
+    }
     const GxTask* __restrict__ Tp = A.plan.tasks + task_id;
     const int n = Tp->n, n1 = Tp->n1, n2 = Tp->n2, e1 = Tp->e1, np = Tp->npairs_in;  // inner pairs only
     // gradient baseline: the loss is taken at the node's PREDICTED label (explain.py:130), otherwise at label[node] (explain.py:750-753)
@@ -192,9 +202,6 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
     __syncthreads();
     const int dp = sL.dp, D4 = dp / 4;
     const int32_t* __restrict__ lo2gid = A.plan.lo2gid + node_off;
-    const float nn = (float)n * (float)n;
-    const float ent_over_nn = hp.c_ent / nn;
-    const float lap_over_nn = hp.c_lap / nn;
 
     // ------------------------------------------------------------------ load
     {
@@ -344,15 +351,19 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
     // lane groups: GW lanes per row
     Grp G;
     {
-      int gw = D4 > H4 ? D4 : H4;
+      int gw = kNarrow ? H4 : (D4 > H4 ? D4 : H4);
       gw = gw > (EMB / 4) ? gw : (EMB / 4);
       G.GW = gw; G.epi = 32 / gw; G.lane = lane; G.grp = lane / gw; G.q = lane - G.grp * gw; G.gbase = G.grp * gw;
     }
     const int epi = G.epi, q = G.q;
 
     // ------------------------------------------------------------------ epochs
-    long long tF1 = 0, tF2 = 0, tS = 0, tB2 = 0, tB1 = 0, tP = 0, tl = clock64();
-#define GX_MARK(acc) if (A.dbg != nullptr && warp == 0) { const long long c_ = clock64(); acc += c_ - tl; tl = c_; }
+    // phase timers (tools/phase_timers.py): kept in shared memory, so that they take no registers in the epoch loop
+    if (A.dbg != nullptr && tid == 0) {
+      for (int k = 0; k < 6; ++k) s_clk[k] = 0;
+      s_clk[6] = clock64();
+    }
+#define GX_MARK(k) if (A.dbg != nullptr && tid == 0) { const long long c_ = clock64(); s_clk[k] += c_ - s_clk[6]; s_clk[6] = c_; }
     for (int it = 1; it <= hp.iters; ++it) {
       // ---- F1: rows [0,n2): U = A_m X ; Y1 = (U . sF) W1 + b1 ; row normalise            (models.py:70-78)
       {
@@ -375,8 +386,8 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
           }
           __syncwarp();
           float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (act && q < H4) y = group_dense(zs + G.gbase * 4, D4, W1s, HS, q, ld4(bs + 4 * q));
-          const float ss = group_sum(y.x * y.x + y.y * y.y + y.z * y.z + y.w * y.w, G);
+          if (act && q < H4) y = group_dense<kF4>(zs + G.gbase * 4, D4, W1s, HS, q, ld4(bs + 4 * q));
+          const float ss = group_sum<kGW>(y.x * y.x + y.y * y.y + y.z * y.z + y.w * y.w, G);
           const float qn = fmaxf(sqrtf(ss), 1e-12f);  // F.normalize(p=2, dim=2), eps 1e-12
           const float rq = 1.0f / qn;   // one division per row; the row is scaled by (and the backward reuses) the reciprocal
           if (act && q < H4) peer.st4(Yh1 + i * HS + 4 * q, make_float4(y.x * rq, y.y * rq, y.z * rq, y.w * rq));
@@ -385,7 +396,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         }
       }
       phase_sync<CS>();
-      GX_MARK(tF1)
+      GX_MARK(0)
       // ---- F2: rows [0,n1): Y2 = (A_m relu(Yh1)) W2 + b2 ; row normalise
       {
         const IdxT* const irp = reinterpret_cast<const IdxT*>(base + sL.irp);
@@ -403,7 +414,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
           __syncwarp();
           float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
           if (act && q < H4) y = group_dense(zs + G.gbase * 4, H4, W2s, HS, q, ld4(bs + HID + 4 * q));
-          const float ss = group_sum(y.x * y.x + y.y * y.y + y.z * y.z + y.w * y.w, G);
+          const float ss = group_sum<kGW>(y.x * y.x + y.y * y.y + y.z * y.z + y.w * y.w, G);
           const float qn = fmaxf(sqrtf(ss), 1e-12f);
           const float rq = 1.0f / qn;
           if (act && q < H4) peer.st4(Yh2 + i * HS + 4 * q, make_float4(y.x * rq, y.y * rq, y.z * rq, y.w * rq));
@@ -412,7 +423,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         }
       }
       phase_sync<CS>();
-      GX_MARK(tF2)
+      GX_MARK(1)
       // ---- S: row r (= level-order id 0): layer 3, readout, softmax, -log p[gt], layer-3 backward
       if (warp == 0) {
         const IdxT* const irp = reinterpret_cast<const IdxT*>(base + sL.irp);
@@ -435,7 +446,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         }
       }
       __syncthreads();
-      GX_MARK(tS)
+      GX_MARK(2)
       // ---- B2: rows {r} U N(r): dYh2 = dEmb2 (row r) + a[r,j] dZ3 (j in N(r)), relu', normalise', dZ2 = dY2 W2^T
       {
         const IdxT* const irp = reinterpret_cast<const IdxT*>(base + sL.irp);
@@ -467,7 +478,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
             dy.z = yh.z > 0.f ? coef * g4.z : 0.f;
             dy.w = yh.w > 0.f ? coef * g4.w : 0.f;
           }
-          const float sdot = group_sum(yh.x * dy.x + yh.y * dy.y + yh.z * dy.z + yh.w * dy.w, G);
+          const float sdot = group_sum<kGW>(yh.x * dy.x + yh.y * dy.y + yh.z * dy.z + yh.w * dy.w, G);
           if (act && q < H4) {
             const float rq = q2[j];   // 1 / max(|Y2[j]|, eps)
             st4(zs + lane * 4, make_float4((dy.x - yh.x * sdot) * rq, (dy.y - yh.y * sdot) * rq,
@@ -480,7 +491,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         }
       }
       __syncthreads();
-      GX_MARK(tB2)
+      GX_MARK(3)
       // ---- B1: rows [0,n2): dH1 = A_m^T dZ2 (only columns < n1 carry gradient), relu', normalise',
       //          dZ1 = dY1 W1^T, dL/dsF partial, dZ1 (.) sF kept for the edge dots
       {
@@ -506,7 +517,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
             dy.x = yh.x > 0.f ? dh.x : 0.f; dy.y = yh.y > 0.f ? dh.y : 0.f;
             dy.z = yh.z > 0.f ? dh.z : 0.f; dy.w = yh.w > 0.f ? dh.w : 0.f;
           }
-          const float sdot = group_sum(yh.x * dy.x + yh.y * dy.y + yh.z * dy.z + yh.w * dy.w, G);
+          const float sdot = group_sum<kGW>(yh.x * dy.x + yh.y * dy.y + yh.z * dy.z + yh.w * dy.w, G);
           if (act && q < H4) {
             const float rq = q1[i];   // 1 / max(|Y1[i]|, eps)
             st4(zs + lane * 4, make_float4((dy.x - yh.x * sdot) * rq, (dy.y - yh.y * sdot) * rq,
@@ -537,7 +548,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         __syncwarp();
       }
       phase_sync<CS>();
-      GX_MARK(tB1)
+      GX_MARK(4)
       if (A.dbg != nullptr && it == 1 && qi == 0 && crank == 0) {   // debug: [header 16 floats][whole task slab]
         if (tid == 0) {
           A.dbg[0] = (float)sL.total_words; A.dbg[1] = (float)sL.X; A.dbg[2] = (float)sL.U; A.dbg[3] = (float)sL.Yh1;
@@ -568,6 +579,9 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         const float2 tab = __ldg(hp.adam_tab + (it - 1));
         const float step = tab.x, bc2s = tab.y, bc2s_inv = 1.0f / tab.y;
         const bool last = (it == hp.out_iter);   // the mask built after this update is the one the reference returns
+        const float nn = (float)n * (float)n;      // (formed here rather than once per task: nothing has to stay live across the epoch)
+        const float ent_over_nn = hp.c_ent / nn;
+        const float lap_over_nn = hp.c_lap / nn;
         // feature mask: dL/dF = sF(1-sF) (sum_i dZ1[i] U[i] + feat_size/d) ; Adam (explain.py:766, train_utils.py:10)
         // (done by the LAST warps of the CTA: the first ones carry the most pair work below, and a warp whose first lanes run this
         //  serial update would hold back its 32 pairs)
@@ -600,8 +614,8 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
             if (p + pstride < np) pxn = PX[p + pstride];
             const int i = px.x & 0xffffu, j = px.x >> 16;
             float gij = 0.f, gji = 0.f;
-            if (i < n2) gij += dot_v4(dZ1s + i * dp, X + j * dp, D4);
-            if (j < n2) gji += dot_v4(dZ1s + j * dp, X + i * dp, D4);
+            if (i < n2) gij += dot_v4<kF4>(dZ1s + i * dp, X + j * dp, D4);
+            if (j < n2) gji += dot_v4<kF4>(dZ1s + j * dp, X + i * dp, D4);
             if (i < n1) gij += dot_relu_v4(dZ2 + i * HS, Yh1 + j * HS, H4);
             if (j < n1) gji += dot_relu_v4(dZ2 + j * HS, Yh1 + i * HS, H4);
             if (i == 0) gij += dot_relu_v4(dZ3, Yh2 + j * HS, H4);
@@ -624,8 +638,8 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
             trS += Sv.x + Sv.y; trH += bern_entropy(Sv.x) + bern_entropy(Sv.y);
             trL += 0.5f * (Sv.x + Sv.y) * yd * yd;
           }
-          if (i < n2) Gd += dot_v4(dZ1s + i * dp, X + j * dp, D4);
-          if (j < n2) Gd += dot_v4(dZ1s + j * dp, X + i * dp, D4);
+          if (i < n2) Gd += dot_v4<kF4>(dZ1s + i * dp, X + j * dp, D4);
+          if (j < n2) Gd += dot_v4<kF4>(dZ1s + j * dp, X + i * dp, D4);
           if (i < n1) Gd += dot_relu_v4(dZ2 + i * HS, Yh1 + j * HS, H4);
           if (j < n1) Gd += dot_relu_v4(dZ2 + j * HS, Yh1 + i * HS, H4);
           if (i == 0) Gd += dot_relu_v4(dZ3, Yh2 + j * HS, H4);
@@ -668,19 +682,20 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_node_kernel(const Expla
         const float* const tr = s_tr + (NT / 32) * CS * 4;
         row[0] = sS; row[1] = tr[0]; row[2] = sH; row[3] = sLp; row[4] = sD; row[5] = tr[2]; row[6] = 0.f; row[7] = tr[1];
       }
-      GX_MARK(tP)
+      GX_MARK(5)
     }
     if (A.dbg != nullptr && tid == 0 && qi == 0 && crank == 0) {
       float* o = A.dbg + (1 << 19);
-      o[0] = (float)tF1; o[1] = (float)tF2; o[2] = (float)tS; o[3] = (float)tB2; o[4] = (float)tB1; o[5] = (float)tP;
+      for (int k = 0; k < 6; ++k) o[k] = (float)s_clk[k];
       o[6] = (float)n; o[7] = (float)n1; o[8] = (float)n2; o[9] = (float)np; o[10] = (float)e1; o[11] = (float)nthreads;
+      o[12] = kNarrow ? 1.f : 0.f;   // which instantiation ran (tests/test_gpu_node_narrow.py)
     }
     if (A.dbg != nullptr && tid == 0 && crank == 0) {
       unsigned long long t_end_ns; unsigned smid;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_end_ns));
       asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
       unsigned long long* tl64 = reinterpret_cast<unsigned long long*>(A.dbg + (1 << 19) + 64);
-      tl64[3 * task_id + 0] = t_start_ns; tl64[3 * task_id + 1] = t_end_ns; tl64[3 * task_id + 2] = ((unsigned long long)smid << 32) | (unsigned)nthreads;
+      tl64[3 * task_id + 0] = (unsigned long long)s_clk[7]; tl64[3 * task_id + 1] = t_end_ns; tl64[3 * task_id + 2] = ((unsigned long long)smid << 32) | (unsigned)nthreads;
     }
     phase_sync<CS>();
   }
@@ -777,9 +792,9 @@ outer_pairs_kernel(const GxHparamsDev hp, const GxGraphDev g, const GxPlanArrays
   }
 }
 
-template <typename IdxT, int HID, int EMB, int NT, bool kTrace, int CS>
+template <typename IdxT, int HID, int EMB, int NT, bool kTrace, int CS, bool kNarrow>
 cudaError_t launch_one_t(const GxExplainLaunch& cfg, const ExplainArgs& args, cudaStream_t s) {
-  auto kern = explain_node_kernel<IdxT, HID, EMB, NT, kTrace, CS>;
+  auto kern = explain_node_kernel<IdxT, HID, EMB, NT, kTrace, CS, kNarrow>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cfg.smem_bytes);
   if (e != cudaSuccess) return e;
   // every launch class asks for the largest shared-memory carveout: CTAs of different classes (= different kernels / footprints) can then
@@ -802,10 +817,10 @@ cudaError_t launch_one_t(const GxExplainLaunch& cfg, const ExplainArgs& args, cu
   lc.attrs = at; lc.numAttrs = 1;
   return cudaLaunchKernelEx(&lc, kern, args);
 }
-template <typename IdxT, int HID, int EMB, int NT, int CS>
+template <typename IdxT, int HID, int EMB, int NT, int CS, bool kNarrow = false>
 cudaError_t launch_one(const GxExplainLaunch& cfg, const ExplainArgs& args, cudaStream_t s) {
-  if (args.x.trace != nullptr) return launch_one_t<IdxT, HID, EMB, NT, true, CS>(cfg, args, s);
-  return launch_one_t<IdxT, HID, EMB, NT, false, CS>(cfg, args, s);
+  if (args.x.trace != nullptr) return launch_one_t<IdxT, HID, EMB, NT, true, CS, kNarrow>(cfg, args, s);
+  return launch_one_t<IdxT, HID, EMB, NT, false, CS, kNarrow>(cfg, args, s);
 }
 
 template <int HID, int EMB>
@@ -814,8 +829,12 @@ cudaError_t launch_dims(const GxExplainLaunch& cfg, const ExplainArgs& args, cud
   if (cfg.cluster == 4) return launch_one<uint16_t, HID, EMB, 512, 4>(cfg, args, s);
   if (cfg.cluster == 2) return launch_one<uint16_t, HID, EMB, 512, 2>(cfg, args, s);
   if (cfg.cluster != 1) return cudaErrorInvalidValue;
-  if (cfg.threads <= 256) return launch_one<uint16_t, HID, EMB, 256, 1>(cfg, args, s);
-  return launch_one<uint16_t, HID, EMB, 512, 1>(cfg, args, s);
+  // inputs no wider than the hidden width take the instantiation with the lane-group shape fixed at compile time;
+  // GNNX_NODE_GENERIC=1 (GX_HP_NODE_GENERIC) keeps every task on the run-time-shape code, for tests and A/B runs
+  const bool narrow = HID == EMB && 4 * ((args.m.d + 3) / 4) <= HID && (args.hp.flags & GX_HP_NODE_GENERIC) == 0;
+  if (cfg.threads <= 256)
+    return narrow ? launch_one<uint16_t, HID, EMB, 256, 1, true>(cfg, args, s) : launch_one<uint16_t, HID, EMB, 256, 1>(cfg, args, s);
+  return narrow ? launch_one<uint16_t, HID, EMB, 512, 1, true>(cfg, args, s) : launch_one<uint16_t, HID, EMB, 512, 1>(cfg, args, s);
 }
 
 }  // namespace

@@ -119,6 +119,7 @@ struct GxHparamsDev {
 };
 
 #define GX_HP_IEEE_EDGE 1  // edge phase with IEEE exp/div/sqrt instead of the hardware approximations (test knob)
+#define GX_HP_NODE_GENERIC 2   // explain_node.cu: never the narrow instantiation (test / A-B knob)
 
 // Optional trace / optimiser-state buffers of gx_explain_io (device pointers, nullptr = unused).
 struct GxExtra {

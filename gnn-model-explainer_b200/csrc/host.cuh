@@ -70,6 +70,7 @@ struct gx_handle {
   int exclusive_topk = 30;    // GNNX_EXCLUSIVE_TOPK: tasks of the 2-per-SM class that may get an SM of their own (syn1 sweep, DESIGN section 6)
   bool host_timing = false;   // GNNX_HOST_TIMING=1: stderr breakdown of the host side (tools/)
   bool ieee_edge = false;     // test knob (gx_debug_ieee_edge / GNNX_IEEE_EDGE): IEEE arithmetic in the edge phase
+  bool node_generic = false;  // test / A-B knob (GNNX_NODE_GENERIC=1): explain_node.cu keeps the run-time lane-group shape for every input width
   int gang_override = 0;      // test knob (gx_debug_set_gang / GNNX_GANG): CTAs per task of explain_gang.cu, 0 = automatic, -1 = explain_stream.cu
   int cluster_size = 1;       // gx_debug_set_cluster / GNNX_CLUSTER_SIZE: 1 = never (default: results independent of the batch composition), 0 = automatic, 2 / 4 = forced
   int64_t cluster_cost = 0;   // GNNX_CLUSTER_COST
