@@ -186,6 +186,25 @@ def philox_m0(seed, key, num_slots, n):
 # ----------------------------------------------------------------------------------------------
 
 
+_POOL = [None]
+
+
+def max_pool(outs):
+    """The graph readout's per-layer max over rows (models.py:283,293,304): torch.max, whose backward routes each column's gradient to
+    its first maximal row.  Every graph-mode port pools here; set_pool(fn) makes fn(outs) pool instead (tests/pool_oracle.py forces and
+    records those arg-max choices)."""
+    import torch
+    if _POOL[0] is not None:
+        return _POOL[0](outs)
+    return [torch.max(o, dim=1)[0] for o in outs]
+
+
+def set_pool(fn):
+    """Installs fn (None: torch.max) as max_pool's readout; returns the previous one."""
+    prev, _POOL[0] = _POOL[0], fn
+    return prev
+
+
 def _gcn_forward_torch(x, adj, W, graph_mode, bn=False):
     """models.py:58-80 (GraphConv.forward), :230-267 (gcn_forward), :363-376 (node readout),
     :269-316 (graph readout).  x (1,n,d), adj (1,n,n).  Any number of layers (len(W["conv_w"]) =
@@ -210,7 +229,7 @@ def _gcn_forward_torch(x, adj, W, graph_mode, bn=False):
         outs.append(y)
         h = y
     if graph_mode:
-        pooled = [torch.max(o, dim=1)[0] for o in outs]            # models.py:283,293,304
+        pooled = max_pool(outs)                                    # models.py:283,293,304
         emb = torch.cat(pooled, dim=1)                             # models.py:309
         return F.linear(emb, W["pred_w"], W["pred_b"])             # (1,C)
     emb = torch.cat(outs, dim=2)                                   # models.py:260

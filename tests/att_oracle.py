@@ -50,7 +50,7 @@ def gcn_forward_att_torch(x, adj, W, graph_mode, bn=False):
         outs.append(y)
         h = y
     if graph_mode:
-        emb = torch.cat([torch.max(o, dim=1)[0] for o in outs], dim=1)
+        emb = torch.cat(O.max_pool(outs), dim=1)
         return F.linear(emb, W["pred_w"], W["pred_b"])
     return F.linear(torch.cat(outs, dim=2), W["pred_w"], W["pred_b"])
 

@@ -72,7 +72,7 @@ def gcn_forward(x, adj, W, graph_mode, bn=False):
         outs.append(y)
         h = y
     if graph_mode:
-        return pred_model(torch.cat([torch.max(o, dim=1)[0] for o in outs], dim=1), W)
+        return pred_model(torch.cat(O.max_pool(outs), dim=1), W)
     return pred_model(torch.cat(outs, dim=2), W)
 
 

@@ -11,10 +11,12 @@ import torch
 
 import gnnx
 import gnnx_oracle as O
+import pool_oracle as PO
 import util
 import wide_oracle as WO
 from gnnx import _abi
 from test_gpu_deep import GG, GX_ERR_UNSUPPORTED, _args, _check, _graph_setup, _hp, _m0, _node_setup, _ohp, _state_dict, _sub, random_model
+from test_oracle_pool_ties import NEAR_TIES
 from test_oracle_wide_layers import GOLDEN, case_weights, golden_cases
 
 pytestmark = pytest.mark.gpu
@@ -354,7 +356,9 @@ def test_wide_layers_sharded_explain_matches_explain_nodes(tmp_path):
 # ---------------------------------------------------------------------------------------------------------- the unmodified reference
 @pytest.mark.parametrize("case,mode", golden_cases(), ids=lambda c: str(c))
 def test_wide_layers_match_reference_golden(case, mode):
-    """Every node and graph of tests/golden/wide_layers_golden.npz within max(1e-4, 3 x the reference's own spread)."""
+    """Every node and graph of tests/golden/wide_layers_golden.npz within max(1e-4, 3 x the reference's own spread) of the reference's
+    mask or, for the graphs with a near tie in their max-pool readout (tests/test_oracle_pool_ties.py), of the nearest admissible
+    trajectory (tests/pool_oracle.py)."""
     g = np.load(GOLDEN)
     k = lambda s_: g["%s_%s" % (case, s_)]
     w = case_weights(g, case)
@@ -393,9 +397,12 @@ def test_wide_layers_match_reference_golden(case, mode):
             Dm[rc[gi]] = out[edge_off[gi]:edge_off[gi + 1]]
             ei, ej = np.nonzero(GG["adj"][gi])
             tol = max(1e-4, 3 * float(g["%s_g%d_spread" % (case, gi)]))
-            if (case, gi) == ("graphs_h256", 8):
-                tol = 5e-4   # 3.6e-4 with either product: an open finding (DESIGN section 15), the fp64 specification is at 1.5e-7
             err = util.rel_l2(Dm[ei, ej], g["%s_g%d_mask" % (case, gi)])
+            if gi in NEAR_TIES.get(("wide_layers", case), {}):   # a sub-ulp arg-max margin: the nearest admissible trajectory
+                A = np.asarray(GG["adj"][gi], np.float64)
+                err = PO.nearest_admissible(Dm[ei, ej], g["%s_g%d_mask" % (case, gi)], A, GG["feat"][gi].astype(np.float32),
+                                            int(GG["label"][gi]), w, O.draw_m0(n, seed=int(GG["g%d_seed" % gi])),
+                                            O.default_hparams(num_epochs=int(k("epochs")), opt=str(k("opt"))), bn)
             assert err <= tol, (case, gi, err, tol)
     eng.close()
 
