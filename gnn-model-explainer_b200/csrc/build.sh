@@ -7,7 +7,7 @@ OUT="${GNNX_BUILD_OUT:-$HERE/../gnnx/lib}"   # GNNX_BUILD_OUT + GNNX_NVCC_EXTRA:
 mkdir -p "$OUT"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -I$ROOT/include -I$HERE ${GNNX_NVCC_EXTRA}"
-SRCS="api node_mode graph_mode unconstrained khop explain_node explain_graph explain_stream explain_gang explain_var explain_dense forward trace denoise comm"
+SRCS="api node_mode graph_mode unconstrained khop explain_node explain_graph explain_stream explain_gang explain_var explain_dense forward trace denoise comm densify_graphs"
 HEADERS=("$ROOT/include/gnnx.h" "$HERE"/*.cuh)
 for f in $SRCS; do
   stale=0

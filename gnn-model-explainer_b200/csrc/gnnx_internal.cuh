@@ -463,3 +463,6 @@ cudaError_t gx_launch_offedge_graphs(const GxHparamsDev& hp, const GxPlanArrays&
                                      const float* m0_dense, double* out, cudaStream_t s);
 cudaError_t gx_launch_densify(const GxPlanArrays& plan, int count, const int64_t* dense_off,
                               const float* edge_mask, double* out, cudaStream_t s);
+// densify_graphs.cu: gids[count] and val_off[count] (start of graph t's packed slots in values) are device arrays
+cudaError_t gx_launch_densify_graphs(const GxGraphBatchDev& gb, const int32_t* gids, int count, const int64_t* val_off,
+                                     const float* values, double* out, cudaStream_t s);

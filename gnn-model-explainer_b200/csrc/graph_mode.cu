@@ -1,5 +1,6 @@
 // graph_mode.cu -- graph classification on the host side of libgnnx.so: the padded graph batch, gx_plan_graphs (one task per graph,
-// sorted into launch classes by shared-memory footprint) and gx_explain_graphs.
+// sorted into launch classes by shared-memory footprint), gx_explain_graphs, and the graph-list helpers of a sharded run: gx_count_graphs
+// and gx_densify_graphs (its kernel: densify_graphs.cu).
 #include <string.h>
 
 #include <algorithm>
@@ -15,6 +16,23 @@ namespace {
 constexpr int kGraphCap[] = {18 * 1024, 27 * 1024, 36 * 1024, 44 * 1024, 80 * 1024, 226 * 1024};
 constexpr int kNumGraphClasses = sizeof(kGraphCap) / sizeof(kGraphCap[0]);
 constexpr int kGraphThreads = 128;
+
+// Rows of graph g that have an edge, and its directed edges: the task size of gx_plan_graphs and of gx_count_graphs.
+void graph_counts(const gx_handle* h, int g, int* active, int32_t* edges) {
+  const int nf = h->gb.max_nodes;
+  const int32_t* rp = h->gb_h_rowptr.data() + (int64_t)g * nf;
+  int na = 0;
+  for (int i = 0; i < nf; ++i) na += rp[i + 1] > rp[i] ? 1 : 0;
+  *active = na;
+  *edges = rp[nf] - rp[0];
+}
+
+// The ids of a graph list: GX_OK when every id names a graph of the uploaded batch.
+int check_graph_list(const gx_handle* h, const char* who, const int32_t* graph_ids, int32_t count) {
+  for (int t = 0; t < count; ++t)
+    if (graph_ids[t] < 0 || graph_ids[t] >= h->gb.num_graphs) { gx_set_error("%s: graph %d out of range", who, graph_ids[t]); return GX_ERR_INVALID; }
+  return GX_OK;
+}
 
 }  // namespace
 
@@ -71,13 +89,12 @@ int gx_plan_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int64_
   for (int t = 0; t < count; ++t) {
     const int g = graph_ids[t];
     if (g < 0 || g >= h->gb.num_graphs) { gx_set_error("gx_plan_graphs: graph %d out of range", g); return GX_ERR_INVALID; }
-    const int32_t* rp = h->gb_h_rowptr.data() + (int64_t)g * nf;
     GxTask& T = h->tasks[t];
     memset(&T, 0, sizeof(T));
     int na = 0;
-    for (int i = 0; i < nf; ++i) na += rp[i + 1] > rp[i] ? 1 : 0;
+    graph_counts(h, g, &na, &T.e_d);
     T.node = g; T.n = na; T.n1 = na; T.n2 = na;
-    T.e_d = rp[nf] - rp[0]; T.e1 = T.e_d; T.npairs = T.e_d / 2; T.npairs_in = T.npairs;
+    T.e1 = T.e_d; T.npairs = T.e_d / 2; T.npairs_in = T.npairs;
     T.gt_label = h->gb_h_label[g]; T.n_norm = nf; T.flags = na < nf ? 1 : 0;
     T.node_off = tn; T.rp_off = tn + t; T.edge_off = te; T.pair_off = tp;
     if (!h->m.variant) {   // the tuned kernel (explain_graph.cu) keeps a graph in shared memory with 16-bit indices
@@ -193,6 +210,53 @@ int gx_explain_graphs(gx_handle* h, const gx_hparams* hp, gx_memspace space, con
 
 int gx_explain_graphs_ex(gx_handle* h, const gx_hparams* hp, gx_memspace space, const gx_explain_io* io) {
   return explain_graphs_impl(h, hp, space, io);
+}
+
+int gx_count_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int32_t* n_out, int32_t* e_out) {
+  if (!h || (count > 0 && (!graph_ids || !n_out || !e_out))) { gx_set_error("gx_count_graphs: NULL argument"); return GX_ERR_INVALID; }
+  if (!h->has_batch) { gx_set_error("gx_count_graphs: call gx_set_graph_batch_csr first"); return GX_ERR_INVALID; }
+  if (count < 0) { gx_set_error("gx_count_graphs: count < 0"); return GX_ERR_INVALID; }
+  const int rc = check_graph_list(h, "gx_count_graphs", graph_ids, count);
+  if (rc != GX_OK) return rc;
+  for (int t = 0; t < count; ++t) graph_counts(h, graph_ids[t], &n_out[t], &e_out[t]);
+  return GX_OK;
+}
+
+int gx_densify_graphs(gx_handle* h, gx_memspace space, const int32_t* graph_ids, int32_t count, const float* values, double* out) {
+  if (!h || (count > 0 && (!graph_ids || !out))) { gx_set_error("gx_densify_graphs: NULL argument"); return GX_ERR_INVALID; }
+  if (!h->has_batch) { gx_set_error("gx_densify_graphs: call gx_set_graph_batch_csr first"); return GX_ERR_INVALID; }
+  if (count < 0) { gx_set_error("gx_densify_graphs: count < 0"); return GX_ERR_INVALID; }
+  int rc = check_graph_list(h, "gx_densify_graphs", graph_ids, count);
+  if (rc != GX_OK || count == 0) return rc;
+  std::vector<int64_t> val_off(count + 1, 0);
+  for (int t = 0; t < count; ++t) {
+    int na;
+    int32_t ed;
+    graph_counts(h, graph_ids[t], &na, &ed);
+    val_off[t + 1] = val_off[t] + ed;
+  }
+  const int64_t total = val_off[count];
+  if (total > 0 && !values) { gx_set_error("gx_densify_graphs: NULL values"); return GX_ERR_INVALID; }
+  const size_t dense = (size_t)count * h->gb.max_nodes * h->gb.max_nodes;
+  GX_CUDA_CHECK(cudaSetDevice(h->device));
+  const size_t b64 = (size_t)count * 8;
+  GX_CUDA_CHECK(h->d_dgraph.reserve(b64 + (size_t)count * 4));
+  char* b = h->d_dgraph.as<char>();
+  GX_CUDA_CHECK(cudaMemcpyAsync(b, val_off.data(), b64, cudaMemcpyHostToDevice, h->stream));
+  GX_CUDA_CHECK(cudaMemcpyAsync(b + b64, graph_ids, (size_t)count * 4, cudaMemcpyHostToDevice, h->stream));
+  const float* v = values;
+  double* o = out;
+  if (space == GX_HOST) {
+    GX_CUDA_CHECK(stage_in(h, h->d_out, values, (size_t)total, &v));
+    GX_CUDA_CHECK(stage_out(h->d_dense, out, dense, &o));
+  }
+  GX_CUDA_CHECK(gx_launch_densify_graphs(h->gb, (const int32_t*)(b + b64), count, (const int64_t*)b, v, o, h->stream));
+  h->launches += 1;
+  if (space == GX_HOST) {
+    GX_CUDA_CHECK(stage_back(h, out, (const double*)o, dense));
+    GX_CUDA_CHECK(cudaStreamSynchronize(h->stream));
+  }
+  return GX_OK;
 }
 
 }  // extern "C"

@@ -111,6 +111,7 @@ struct gx_handle {
   bool has_batch = false, has_gplan = false;
   GxGraphBatchDev gb{};
   DevBuf gb_rowptr, gb_col, gb_feat, gb_label;
+  DevBuf d_dgraph;   // gx_densify_graphs: the value offsets and ids of its list
   std::vector<int32_t> gb_h_rowptr, gb_h_label;
   // slot workspace
   DevBuf ws_buf;

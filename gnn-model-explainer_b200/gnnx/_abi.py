@@ -26,7 +26,7 @@ EXPORTS = [
     "gx_debug_force_stream", "gx_debug_ieee_edge", "gx_debug_set_dump", "gx_debug_set_gang", "gx_debug_set_cluster", "gx_denoise_topk",
     "gx_model_forward", "gx_comm_unique_id", "gx_comm_init", "gx_comm_destroy", "gx_count_nodes", "gx_allgather_masks", "gx_unshard_masks",
     "gx_plan_class_counts", "gx_last_class_ms", "gx_explain_nodes_unconstrained", "gx_explain_graphs_unconstrained",
-    "gx_set_model_att", "gx_set_model_head",
+    "gx_set_model_att", "gx_set_model_head", "gx_count_graphs", "gx_densify_graphs",
 ]
 
 
@@ -109,6 +109,8 @@ def lib():
     L.gx_count_nodes.argtypes = [vp, i32p, C.c_int32, C.c_int32, i32p, i32p]
     L.gx_allgather_masks.argtypes = [vp, f32p, C.c_int64, C.c_int64, f32p]
     L.gx_unshard_masks.argtypes = [vp, f32p, C.c_int32, i64p, i64p, i32p, f32p]
+    L.gx_count_graphs.argtypes = [vp, i32p, C.c_int32, i32p, i32p]
+    L.gx_densify_graphs.argtypes = [vp, C.c_int, i32p, C.c_int32, f32p, vp]
     L.gx_debug_force_stream.argtypes = [vp, C.c_int]
     L.gx_debug_ieee_edge.argtypes = [vp, C.c_int]
     L.gx_debug_set_dump.argtypes = [vp, vp]

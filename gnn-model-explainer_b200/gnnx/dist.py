@@ -10,7 +10,11 @@ gx_allgather_masks; torch.distributed -- gloo in the CPU tests -- when no engine
 the collective.
 
 Per-node arithmetic never crosses a GPU, so results are bit-identical to the 1-GPU run (tests/test_gpu_dist.py,
-tests/test_dist_gloo.py, bench.py "shard_bit_identical")."""
+tests/test_dist_gloo.py, bench.py "shard_bit_identical").
+
+Graph-classification mode is dealt the same way, graph by graph (explain_graphs_sharded): gx_count_graphs gives every graph's payload
+from the batch CSR on the host, and gx_densify_graphs turns the gathered masks into explain_graphs' dense arrays on device
+(tests/test_gpu_dist_graphs.py, tests/test_gpu_dist_graphs_multi.py)."""
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -127,3 +131,44 @@ def explain_nodes_sharded(explainer, node_indices, costs=None, group=None, use_e
         ensure_comm(eng, group)
     values, offsets = allgather_packed(local, e_all, rank, world, costs, group=group, engine=eng if use_engine_comm else None, layout=layout)
     return values, offsets, (plan, pos)
+
+
+def explain_graphs_sharded(explainer, graph_indices, costs=None, group=None, use_engine_comm=True, dense=False):
+    """Explainer(graph_mode=True).explain_graphs across all ranks of the default process group (or `group`): each rank explains its
+    share of the graph list, ONE all-gather delivers every graph's packed masks.  Every model and optimiser explain_graphs accepts.
+    costs: per-graph cost for the balance (default: the graph's directed edges, gx_count_graphs).  The layout is remembered for the list
+    explained last, like explain_nodes_sharded's.
+    Every rank returns (values float32 CUDA tensor, offsets int64 array, (edge_off of this rank's plan or None, this rank's positions));
+    values[offsets[t]:offsets[t+1]] are the masked_adj entries of graph_indices[t] at its CSR slots (row-major).  dense=True appends the
+    (len(graph_indices), max_nodes, max_nodes) float64 CUDA tensor of the dense arrays explain_graphs returns (gx_densify_graphs).
+    With args.gnnx_init = "torch" every rank draws the n^2 normals of EVERY graph of the list (torch's RNG ends as after one process's
+    explain_graphs); "device" draws nothing on the host.  Unlike explain_graphs it prints no per-epoch trace and writes no .npy files."""
+    if not explainer.graph_mode:
+        raise ValueError("explain_graphs_sharded needs an Explainer constructed with graph_mode=True")
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    eng = explainer.engine
+    gids = np.asarray(graph_indices, np.int64)
+    dev = torch.device("cuda", eng.device)
+    key = (gids.tobytes(), world, None if costs is None else np.asarray(costs).tobytes())
+    memo = explainer.__dict__.get("_graph_layout_memo")
+    if memo is None or memo[0] != key:
+        _, e_all = eng.count_graphs(gids)
+        memo = (key, e_all, shard_layout(e_all, world, costs))
+        explainer._graph_layout_memo = memo
+    _, e_all, layout = memo
+    pos = layout[0][rank]
+    hp, init = explainer._hparams()
+    m0_host = None
+    if init == "torch":   # every rank walks the whole list, owning graphs or not, so that torch's RNG is consumed as one process would
+        m0_host = explainer._draw_graph_m0_subset(eng.batch_n, len(gids), pos, [eng.graph_rows_cols(int(g)) for g in gids[pos]])
+    if len(pos):
+        edge_off = eng.plan_graphs(gids[pos])
+        local = eng.explain_graphs_device(hp, None if m0_host is None else torch.from_numpy(m0_host).to(dev))
+    else:
+        edge_off, local = None, torch.zeros(0, dtype=torch.float32, device=dev)
+    if use_engine_comm:
+        ensure_comm(eng, group)
+    values, offsets = allgather_packed(local, e_all, rank, world, costs, group=group, engine=eng if use_engine_comm else None, layout=layout)
+    if dense:
+        return values, offsets, (edge_off, pos), eng.densify_graphs_device(gids, values)
+    return values, offsets, (edge_off, pos)

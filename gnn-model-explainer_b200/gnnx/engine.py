@@ -246,6 +246,7 @@ class Engine:
         te = C.c_int64()
         _abi.check(self._lib.gx_plan_graphs(self._h, _np_ptr(gids), len(gids), _np_ptr(edge_off), C.byref(te)))
         self._graph_count = len(gids)
+        self._graph_total = te.value
         return edge_off
 
     def graph_rows_cols(self, g):
@@ -258,6 +259,44 @@ class Engine:
     def explain_graphs_host(self, hp, m0_edges, edge_mask_out, feat_mask_out=None):
         _abi.check(self._lib.gx_explain_graphs(self._h, C.byref(hp), _abi.GX_HOST, _np_ptr(m0_edges),
                                                _np_ptr(edge_mask_out), _np_ptr(feat_mask_out)))
+
+    def explain_graphs_device(self, hp, m0=None, out=None):
+        """The planned graphs with DEVICE buffers (gx_explain_graphs, GX_DEVICE): m0 (optional torch.float32 CUDA tensor, GX_INIT_M0)
+        -> edge masks as a torch.float32 CUDA tensor [total_edges]; asynchronous on the engine's stream."""
+        import torch
+        te = self._graph_total
+        if out is None:
+            out = torch.empty(max(te, 1), dtype=torch.float32, device=torch.device("cuda", self.device))
+        _abi.check(self._lib.gx_explain_graphs(self._h, C.byref(hp), _abi.GX_DEVICE, C.c_void_p(m0.data_ptr() if m0 is not None else None),
+                                               C.c_void_p(out.data_ptr()), None))
+        return out[:te]
+
+    def count_graphs(self, graph_ids):
+        """(n[count], e_d[count]) of every listed graph of the uploaded batch without building a plan (gx_count_graphs): its rows with
+        an edge and its directed edges."""
+        gids = _i32c(graph_ids)
+        n = np.zeros(len(gids), np.int32); e = np.zeros(len(gids), np.int32)
+        _abi.check(self._lib.gx_count_graphs(self._h, _np_ptr(gids), len(gids), _np_ptr(n), _np_ptr(e)))
+        return n, e
+
+    def densify_graphs_device(self, graph_ids, values, out=None):
+        """gx_densify_graphs on device: the packed float32 masks of the listed graphs in list order (CUDA tensor) -> float64 CUDA tensor
+        (len(graph_ids), max_nodes, max_nodes), zero outside each graph's edges."""
+        import torch
+        gids = _i32c(graph_ids)
+        n = self.batch_n
+        if out is None:
+            out = torch.empty((len(gids), n, n), dtype=torch.float64, device=values.device)
+        _abi.check(self._lib.gx_densify_graphs(self._h, _abi.GX_DEVICE, _np_ptr(gids), len(gids),
+                                               C.c_void_p(values.data_ptr() if values.numel() else None), C.c_void_p(out.data_ptr())))
+        return out
+
+    def densify_graphs_host(self, graph_ids, values):
+        """The same with host buffers: numpy float32 values -> numpy float64 (len(graph_ids), max_nodes, max_nodes)."""
+        gids, values = _i32c(graph_ids), _f32c(values)
+        out = np.empty((len(gids), self.batch_n, self.batch_n), np.float64)
+        _abi.check(self._lib.gx_densify_graphs(self._h, _abi.GX_HOST, _np_ptr(gids), len(gids), _np_ptr(values), _np_ptr(out)))
+        return out
 
     # ---------------------------------------------------------------- hot path
     def make_hparams(self, num_epochs=100, lr=0.1, init=_abi.GX_INIT_M0, seed=0, **over):

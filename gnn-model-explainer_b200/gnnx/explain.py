@@ -253,6 +253,23 @@ class Explainer:
                 np.take(M.numpy().reshape(-1), flat[plan.edge_off[t]:plan.edge_off[t + 1]], out=m0[plan.edge_off[t]:plan.edge_off[t + 1]])
         return m0
 
+    @staticmethod
+    def _draw_graph_m0_subset(n, num_graphs, positions, rows_cols):
+        """Graph mode's counterpart for sharded runs: walk the WHOLE graph list (num_graphs entries) drawing FloatTensor(n, n).normal_(1,
+        std) per graph, n = the padded size, exactly as _explain_graph_batch does, and keep M[rows, cols] of the entries this rank owns
+        (`positions`, ascending; rows_cols[i] = (rows, cols) of positions[i]'s graph in slot order), concatenated -> float32.  torch's
+        global RNG ends where one process's explain_graphs of the same list leaves it, whatever the rank owns."""
+        std = torch.nn.init.calculate_gain("relu") * math.sqrt(2.0 / (n + n))
+        mine = {int(p): i for i, p in enumerate(positions)}
+        parts = [None] * len(mine)
+        for p in range(int(num_graphs)):
+            M = torch.FloatTensor(n, n).normal_(1.0, std)
+            i = mine.get(p)
+            if i is not None:
+                rows, cols = rows_cols[i]
+                parts[i] = M.numpy()[rows, cols]
+        return np.concatenate(parts).astype(np.float32, copy=False) if parts else np.zeros(0, np.float32)
+
     def _explain_batch(self, node_indices, graph_idx=0, model="exp", unconstrained=False):
         if model not in ("exp", "grad"):
             raise NotImplementedError("model=%r (att) is not built" % model)

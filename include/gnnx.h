@@ -309,6 +309,21 @@ int gx_allgather_masks(gx_handle* h, const float* local_dev, int64_t local_float
 int gx_unshard_masks(gx_handle* h, const float* gathered_dev, int32_t items, const int64_t* src_off, const int64_t* dst_off,
                      const int32_t* sizes, float* out_dev);
 
+/* The same for graph-classification mode: explain_graphs (explain.py:356-402) sharded by graph.  Each rank plans and explains its
+ * graphs (gx_plan_graphs / gx_explain_graphs on that subset: the arithmetic of one graph never crosses a GPU, and GX_INIT_PHILOX keys
+ * its draw by the graph id), then gx_allgather_masks + gx_unshard_masks deliver every graph's packed masks in list order.
+ *   gx_count_graphs  : for each listed graph of the uploaded batch, n_out = rows with an edge and e_out = directed edges -- the n and e_d
+ *                      gx_plan_graphs gives that graph -- from the batch CSR on the host, without building a plan, so every rank
+ *                      computes the shard layout alone.  GX_ERR_INVALID for an id out of range or without a batch.
+ *   gx_densify_graphs: the dense return value of explain.py:209-221 for a graph list: `values` holds the packed masks of the listed
+ *                      graphs in list order (graph t's slots = its CSR slice in row-major order, what gx_explain_graphs writes and what
+ *                      the gather returns), out[count * max_nodes * max_nodes] float64 receives one (max_nodes, max_nodes) array per
+ *                      graph, zero outside its edges, bit-identical to a host densify (float -> double is exact).  Both buffers in
+ *                      `space`; graph_ids is a host array.  No plan needed; ids may repeat; count = 0 does nothing; 64-bit indexing
+ *                      (outputs beyond 2^31 elements).  GX_ERR_INVALID for an id out of range or without a batch. */
+int gx_count_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int32_t* n_out, int32_t* e_out);
+int gx_densify_graphs(gx_handle* h, gx_memspace space, const int32_t* graph_ids, int32_t count, const float* values, double* out);
+
 /* GcnEncoderNode.forward on the uploaded graph (models.py:58-80,230-267,363-376): pred[num_nodes * num_classes] = the logits the
  * reference reads from its checkpoint (`cg["pred"]`, explainer_main.py:186-193) and hands to Explainer(pred=...).  Raw adjacency
  * (self loops included), no masks; every model gx_set_model accepts (2 / 3 / 4 layers, --bn). */

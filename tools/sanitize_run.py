@@ -3,7 +3,7 @@
     compute-sanitizer --tool racecheck python tools/sanitize_run.py
 k-hop extraction + shared-memory kernel on a mix of task sizes (syn1: hub node 0 and tiny tasks), the streaming kernel (forced),
 the gradient baseline, graph mode, densify, the off-edge regulariser sums of graph mode, neighbourhood rows, the unconstrained (dense) kernel, attention models, inputs wider than 128
-features (explain_var.cu's wide path), models with 5 to 7 layers.  A few epochs each."""
+features (explain_var.cu's wide path), models with 5 to 7 layers, graph-mode sharding's densify (dist_graphs).  A few epochs each."""
 import os
 import sys
 
@@ -20,7 +20,7 @@ EPOCHS = int(os.environ.get("SAN_EPOCHS", "4"))
 
 
 def main():
-    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster", "dense", "att", "wide"]
+    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster", "dense", "att", "wide", "dist_graphs"]
     fx = util.load_fixture("syn1")
     if "node" in which:
         eng = util.make_engine(fx)
@@ -301,6 +301,23 @@ def main():
                                               np.random.default_rng(0).normal(1.0, 0.2, 4 * n * n).astype(np.float32))
         print("misc ok offedge graphs", float(off.sum()))
         eng.close()
+    if "dist_graphs" in which:   # gx_count_graphs and gx_densify_graphs (densify_graphs.cu) on a repeated id, with max_nodes 41 as well:
+        # every other graph's dense block then starts at an odd double (the scalar head store)
+        g = np.load(util.GOLDEN + "/graphs_golden.npz")
+        for n in (40, 41):
+            adj = np.zeros((12, n, n), np.uint8)
+            adj[:, :40, :40] = g["adj"]
+            eng = gnnx.Engine(0)
+            eng.set_model({k: g[k] for k in util.WKEYS})
+            eng.set_graph_batch(adj, np.pad(g["feat"], ((0, 0), (0, n - 40), (0, 0))), g["label"])
+            gids = [5, 0, 11, 5, 3]
+            eoff = eng.plan_graphs(gids)
+            out = np.zeros(int(eoff[-1]), np.float32)
+            eng.explain_graphs_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=3), None, out)
+            _, e = eng.count_graphs(gids)
+            dense = eng.densify_graphs_host(gids, out)
+            print("dist_graphs ok", n, int(e.sum()), float(dense.sum()))
+            eng.close()
 
 
 if __name__ == "__main__":
