@@ -747,6 +747,36 @@ int gx_denoise_topk(gx_handle* h, gx_memspace space, const float* edge_mask, int
   return GX_OK;
 }
 
+int gx_denoise_topk_edges(gx_handle* h, gx_memspace space, const float* edge_mask, int32_t threshold_num, int32_t cap,
+                          float* out_threshold, int32_t* out_count, int32_t* out_uv, float* out_vals) {
+  if (!h || !edge_mask || !out_threshold || !out_count || !out_uv) { gx_set_error("gx_denoise_topk_edges: NULL argument"); return GX_ERR_INVALID; }
+  if (!h->has_plan) { gx_set_error("gx_denoise_topk_edges: no plan (call gx_plan_nodes)"); return GX_ERR_INVALID; }
+  if (threshold_num < 1 || cap < 1) { gx_set_error("gx_denoise_topk_edges: threshold_num and cap must be >= 1"); return GX_ERR_INVALID; }
+  GX_CUDA_CHECK(cudaSetDevice(h->device));
+  const size_t count = (size_t)h->count, nslots = count * cap;
+  const float* em = edge_mask;
+  float* thr = out_threshold; int32_t* cnt = out_count; int32_t* uv = out_uv; float* vals = out_vals;
+  if (space == GX_HOST) {
+    GX_CUDA_CHECK(stage_in(h, h->d_out, edge_mask, (size_t)h->total_e, &em));
+    GX_CUDA_CHECK(stage_out(h->d_dn_thr, out_threshold, count, &thr));
+    GX_CUDA_CHECK(stage_out(h->d_dn_cnt, out_count, count, &cnt));
+    GX_CUDA_CHECK(stage_out(h->d_dn_slots, out_uv, 2 * nslots, &uv));
+    GX_CUDA_CHECK(stage_out(h->d_dn_vals, out_vals, nslots, &vals));
+  }
+  GX_CUDA_CHECK(cudaMemsetAsync(uv, 0xFF, 2 * nslots * 4, h->stream));   // unused pairs read as (-1, -1)
+  if (vals) GX_CUDA_CHECK(cudaMemsetAsync(vals, 0, nslots * 4, h->stream));
+  GX_CUDA_CHECK(gx_launch_denoise_topk_edges(h->plan, (int)count, em, 2 * threshold_num, cap, thr, cnt, uv, vals, h->stream));
+  h->launches += 1;
+  if (space == GX_HOST) {
+    GX_CUDA_CHECK(stage_back(h, out_threshold, (const float*)thr, count));
+    GX_CUDA_CHECK(stage_back(h, out_count, (const int32_t*)cnt, count));
+    GX_CUDA_CHECK(stage_back(h, out_uv, (const int32_t*)uv, 2 * nslots));
+    GX_CUDA_CHECK(stage_back(h, out_vals, (const float*)vals, nslots));
+    GX_CUDA_CHECK(cudaStreamSynchronize(h->stream));
+  }
+  return GX_OK;
+}
+
 int gx_densify(gx_handle* h, gx_memspace space, const float* edge_mask, double* out) {
   if (!h || !edge_mask || !out) { gx_set_error("gx_densify: NULL argument"); return GX_ERR_INVALID; }
   if (!h->has_plan) { gx_set_error("gx_densify: no plan"); return GX_ERR_INVALID; }

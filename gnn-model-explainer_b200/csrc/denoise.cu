@@ -6,15 +6,31 @@
 // E_t packed values (4 passes of an 8-bit histogram on the float bits: positive floats order like unsigned integers) and an
 // order-preserving compaction -- one CTA per explained node.  It is also the payload policy of the multi-GPU gather for graphs
 // whose full masks cannot be gathered (BASELINE configs[4]: 3.4 GB of masks per 132 nodes; the top-k lists are 132 x 40 entries).
+// The edges mode (gx_denoise_topk_edges) shares the select and the compaction: it keeps the row < col half of the surviving slots
+// and writes them as global (u, v) pairs, so a gathered list needs no plan to be read.
 #include "gnnx_internal.cuh"
 
 namespace {
 
 constexpr int DN_THREADS = 256;
 
+// Row of canonical slot e of a task: the last r with rp[r] <= e (rp = the task's n+1 sub_rowptr entries, rp[0] = 0 <= e < rp[n]).
+__device__ __forceinline__ int slot_row(const int32_t* __restrict__ rp, int n, int e) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (rp[mid] <= e) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// kEdges = false (gx_denoise_topk): out_idx[t*cap + i] = the i-th kept slot (task-local), every kept slot.
+// kEdges = true (gx_denoise_topk_edges): only kept slots with row < col, written as the global pair (nbrs[row], nbrs[col]) at
+// out_idx[(t*cap + i)*2 ..]; the kernels write both directions of an edge with the same bits, so the other half adds nothing.
+template <bool kEdges>
 __global__ void __launch_bounds__(DN_THREADS)
 denoise_topk_kernel(const GxPlanArrays plan, int count, const float* __restrict__ edge_mask, int k2, int cap,
-                    float* __restrict__ out_thr, int32_t* __restrict__ out_cnt, int32_t* __restrict__ out_slots,
+                    float* __restrict__ out_thr, int32_t* __restrict__ out_cnt, int32_t* __restrict__ out_idx,
                     float* __restrict__ out_vals) {
   __shared__ int s_hist[256];
   __shared__ unsigned s_prefix;
@@ -72,9 +88,17 @@ denoise_topk_kernel(const GxPlanArrays plan, int count, const float* __restrict_
     // order-preserving compaction of the slots with value >= threshold
     if (tid == 0) s_base = 0;
     __syncthreads();
+    const int32_t* rp = plan.sub_rowptr + T->rp_off;
+    const int32_t* col = plan.sub_col + T->edge_off;
+    const int32_t* nb = plan.nbrs + T->node_off;
     for (int e0 = 0; e0 < E; e0 += DN_THREADS) {
       const int e = e0 + tid;
-      const bool keep = e < E && v[e] >= thr;
+      bool keep = e < E && v[e] >= thr;
+      int row = 0;
+      if (kEdges && keep) {
+        row = slot_row(rp, T->n, e);
+        keep = row < col[e];
+      }
       const unsigned bal = __ballot_sync(0xffffffffu, keep);
       if (lane == 0) s_wcnt[warp] = __popc(bal);
       __syncthreads();
@@ -83,8 +107,14 @@ denoise_topk_kernel(const GxPlanArrays plan, int count, const float* __restrict_
       if (keep) {
         const int pos = off + __popc(bal & ((1u << lane) - 1u));
         if (pos < cap) {
-          out_slots[(int64_t)t * cap + pos] = e;
-          if (out_vals != nullptr) out_vals[(int64_t)t * cap + pos] = v[e];
+          const int64_t o = (int64_t)t * cap + pos;
+          if (kEdges) {
+            out_idx[2 * o] = nb[row];
+            out_idx[2 * o + 1] = nb[col[e]];
+          } else {
+            out_idx[o] = e;
+          }
+          if (out_vals != nullptr) out_vals[o] = v[e];
         }
       }
       __syncthreads();
@@ -101,6 +131,13 @@ denoise_topk_kernel(const GxPlanArrays plan, int count, const float* __restrict_
 cudaError_t gx_launch_denoise_topk(const GxPlanArrays& plan, int count, const float* edge_mask, int k2, int cap, float* out_thr,
                                    int32_t* out_cnt, int32_t* out_slots, float* out_vals, cudaStream_t s) {
   const int grid = count < GX_GRID_CAP ? count : GX_GRID_CAP;
-  denoise_topk_kernel<<<grid, DN_THREADS, 0, s>>>(plan, count, edge_mask, k2, cap, out_thr, out_cnt, out_slots, out_vals);
+  denoise_topk_kernel<false><<<grid, DN_THREADS, 0, s>>>(plan, count, edge_mask, k2, cap, out_thr, out_cnt, out_slots, out_vals);
+  return cudaGetLastError();
+}
+
+cudaError_t gx_launch_denoise_topk_edges(const GxPlanArrays& plan, int count, const float* edge_mask, int k2, int cap, float* out_thr,
+                                         int32_t* out_cnt, int32_t* out_uv, float* out_vals, cudaStream_t s) {
+  const int grid = count < GX_GRID_CAP ? count : GX_GRID_CAP;
+  denoise_topk_kernel<true><<<grid, DN_THREADS, 0, s>>>(plan, count, edge_mask, k2, cap, out_thr, out_cnt, out_uv, out_vals);
   return cudaGetLastError();
 }

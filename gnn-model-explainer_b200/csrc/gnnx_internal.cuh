@@ -446,6 +446,8 @@ cudaError_t gx_launch_outer_pairs(const GxHparamsDev& hp, const GxGraphDev& g, c
                                   const float* m0, float* out_mask, const GxExtra& x, cudaStream_t s);
 cudaError_t gx_launch_denoise_topk(const GxPlanArrays& plan, int count, const float* edge_mask, int k2, int cap, float* out_thr,
                                    int32_t* out_cnt, int32_t* out_slots, float* out_vals, cudaStream_t s);
+cudaError_t gx_launch_denoise_topk_edges(const GxPlanArrays& plan, int count, const float* edge_mask, int k2, int cap, float* out_thr,
+                                         int32_t* out_cnt, int32_t* out_uv, float* out_vals, cudaStream_t s);
 // comm.cu
 struct GxComm;
 int gx_comm_impl_unique_id(char* id128);

@@ -26,7 +26,7 @@ EXPORTS = [
     "gx_debug_force_stream", "gx_debug_ieee_edge", "gx_debug_set_dump", "gx_debug_set_gang", "gx_debug_set_cluster", "gx_denoise_topk",
     "gx_model_forward", "gx_comm_unique_id", "gx_comm_init", "gx_comm_destroy", "gx_count_nodes", "gx_allgather_masks", "gx_unshard_masks",
     "gx_plan_class_counts", "gx_last_class_ms", "gx_explain_nodes_unconstrained", "gx_explain_graphs_unconstrained",
-    "gx_set_model_att", "gx_set_model_head", "gx_count_graphs", "gx_densify_graphs",
+    "gx_set_model_att", "gx_set_model_head", "gx_count_graphs", "gx_densify_graphs", "gx_denoise_topk_edges",
 ]
 
 
@@ -103,6 +103,7 @@ def lib():
     L.gx_offedge_regularisers_graphs.argtypes = [vp, C.POINTER(GxHparams), C.c_int, f32p, vp]
     L.gx_grad_nodes.argtypes = [vp, C.c_int, f32p]
     L.gx_denoise_topk.argtypes = [vp, C.c_int, f32p, C.c_int32, C.c_int32, f32p, i32p, i32p, f32p]
+    L.gx_denoise_topk_edges.argtypes = [vp, C.c_int, f32p, C.c_int32, C.c_int32, f32p, i32p, i32p, f32p]
     L.gx_comm_unique_id.argtypes = [C.c_char_p]
     L.gx_comm_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p]
     L.gx_comm_destroy.argtypes = [vp]

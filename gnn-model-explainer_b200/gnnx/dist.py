@@ -14,7 +14,11 @@ tests/test_dist_gloo.py, bench.py "shard_bit_identical").
 
 Graph-classification mode is dealt the same way, graph by graph (explain_graphs_sharded): gx_count_graphs gives every graph's payload
 from the batch CSR on the host, and gx_densify_graphs turns the gathered masks into explain_graphs' dense arrays on device
-(tests/test_gpu_dist_graphs.py, tests/test_gpu_dist_graphs_multi.py)."""
+(tests/test_gpu_dist_graphs.py, tests/test_gpu_dist_graphs_multi.py).
+
+Graphs whose full masks cannot be gathered (BASELINE configs[4]) deliver denoise_graph's top-k edges instead (explain_nodes_topk_sharded):
+each rank explains its share a chunk at a time and keeps the thresholded edges in global node ids on device (gx_denoise_topk_edges); two
+all-gathers move (threshold, count) per node and 3 words per edge (allgather_topk; tests/test_gpu_topk_edges.py, test_topk_gather_gloo.py)."""
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -172,3 +176,73 @@ def explain_graphs_sharded(explainer, graph_indices, costs=None, group=None, use
     if dense:
         return values, offsets, (edge_off, pos), eng.densify_graphs_device(gids, values)
     return values, offsets, (edge_off, pos)
+
+
+def explain_nodes_topk_sharded(explainer, node_indices, threshold_num=20, chunk_size=None, costs=None, group=None, use_engine_comm=True,
+                               timings=None):
+    """Explainer.explain_nodes_topk across all ranks of the default process group (or `group`), for lists whose full masks cannot be
+    gathered (BASELINE configs[4]: 3.4 GB of masks per 132 nodes).  The nodes are dealt as in explain_nodes_sharded (count_nodes_cached,
+    shard_layout, cost = E_d unless `costs`); each rank runs explain_nodes_topk's chunk loop over its own positions, then TWO all-gathers
+    (allgather_packed: gx_allgather_masks / gx_unshard_masks with the engine's communicator, torch.distributed without it) deliver
+      1. (threshold, count) of every node -- 2 words each, sizes known in advance;
+      2. the kept edges -- 3 words each: u and v bit-cast int32, then the value; the sizes come from gather 1, and the layout keeps the
+         explanation's shards (the same costs, no re-sort by record size).
+    Every rank returns (thr, offsets, uv, vals, positions): thr / offsets / uv / vals exactly as explain_nodes_topk(node_indices) on one
+    GPU, bit for bit; positions = the list entries this rank explained.  With args.gnnx_init = "torch" every rank walks the whole list
+    through torch's RNG once, keeping the normals of its own nodes chunk by chunk.
+    timings (dict or None): per-rank wall seconds of count, plan, m0, explain, topk, gather1, gather2 (synchronising after each phase),
+    the explainer kernels' device seconds (explain_device) and the gathered bytes."""
+    import time
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    eng = explainer.engine
+    if explainer.graph_mode:
+        raise ValueError("explain_nodes_topk_sharded is node mode only")
+    nodes = np.asarray(node_indices, np.int64).reshape(-1)
+    dev = torch.device("cuda", eng.device)
+    t0 = time.perf_counter()
+    n_all, e_all = count_nodes_cached(explainer, nodes)
+    cost = np.asarray(e_all if costs is None else costs)
+    shards = shard_layout(e_all, world, cost)[0]
+    pos = shards[rank]
+    if timings is not None:
+        timings["count"] = timings.get("count", 0.0) + time.perf_counter() - t0
+    thr, cnt, uv, vals = explainer._topk_chunks(nodes, pos, n_all, threshold_num, chunk_size, timings=timings)
+    if use_engine_comm:
+        ensure_comm(eng, group)
+    thr, offsets, uv, vals = allgather_topk(thr, cnt, uv, vals, cost, group=group, engine=eng if use_engine_comm else None, timings=timings)
+    return thr, offsets, uv, vals, pos
+
+
+def allgather_topk(thr, counts, uv, vals, costs, group=None, engine=None, timings=None):
+    """The two all-gathers of explain_nodes_topk_sharded.  This rank's items are the positions shard_layout(costs, world, costs)[0][rank]
+    (ascending) of a list of len(costs) items: thr [k] float32 and counts [k] (host) per item, and the items' records uv [sum counts, 2]
+    int32 and vals [sum counts] float32, item after item (tensors on one device).  Gather 1 moves (threshold, count) of every item, 2 words
+    each; gather 2 moves 3 words per record (u, v bit-cast, value) with sizes from gather 1, in the same shards (layouts from `costs`, not
+    from the record sizes).  Both go through allgather_packed (engine: the library's communicator).
+    Returns (thr [num], offsets int64 [num+1], uv [total, 2], vals [total]) of the whole list in list order, on every rank."""
+    import time
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    costs = np.asarray(costs)
+    num = len(costs)
+    dev = thr.device
+
+    def gathered(key, local, sizes):
+        t1 = time.perf_counter()
+        out, _ = allgather_packed(local, sizes, rank, world, group=group, engine=engine, layout=shard_layout(sizes, world, costs))
+        if timings is not None:
+            if dev.type == "cuda":
+                torch.cuda.synchronize(dev)
+            timings[key] = timings.get(key, 0.0) + time.perf_counter() - t1
+            timings[key + "_bytes"] = timings.get(key + "_bytes", 0) + 4 * int(np.sum(sizes))
+        return out
+
+    # 1. (threshold, count) per item
+    cnt32 = torch.from_numpy(np.ascontiguousarray(counts, np.int32)).to(dev)
+    head = torch.stack([thr.float(), cnt32.view(torch.float32)], 1).reshape(-1)
+    g1 = gathered("gather1", head, np.full(num, 2, np.int64)).view(-1, 2)
+    cnt_all = g1[:, 1].contiguous().view(torch.int32).cpu().numpy().astype(np.int64)
+    # 2. the records, in the same shards
+    rec = torch.cat([uv.contiguous().view(torch.float32), vals.reshape(-1, 1)], 1).reshape(-1)
+    g2 = gathered("gather2", rec, 3 * cnt_all).view(-1, 3)
+    offsets = np.concatenate([[0], np.cumsum(cnt_all)]).astype(np.int64)
+    return g1[:, 0].contiguous(), offsets, g2[:, :2].contiguous().view(torch.int32), g2[:, 2].contiguous()

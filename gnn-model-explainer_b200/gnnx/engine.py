@@ -448,6 +448,31 @@ class Engine:
                                              _np_ptr(thr), _np_ptr(cnt), _np_ptr(slots), _np_ptr(vals)))
         return thr, cnt, slots, vals
 
+    def denoise_topk_edges(self, edge_mask, threshold_num=20, cap=None):
+        """denoise_topk's thresholding of every planned node, delivered as undirected edges in global node ids (gx_denoise_topk_edges):
+        returns (threshold[count], count[count], uv[count,cap,2], vals[count,cap]); node t's kept edges are uv[t, :count[t]] (u < v,
+        ascending), -1 padded.  A numpy edge_mask gives numpy arrays; a CUDA tensor gives CUDA tensors on the same device, asynchronous
+        on the engine's stream.  count[t] > cap when values tie at the threshold: only the first cap edges are written."""
+        count = self._plan_sizes[0]
+        cap = int(cap or threshold_num + 16)
+        if hasattr(edge_mask, "is_cuda") and edge_mask.is_cuda:
+            import torch
+            dev = edge_mask.device
+            em = edge_mask.contiguous()
+            thr = torch.empty(count, dtype=torch.float32, device=dev)
+            cnt = torch.empty(count, dtype=torch.int32, device=dev)
+            uv = torch.empty((count, cap, 2), dtype=torch.int32, device=dev)
+            vals = torch.empty((count, cap), dtype=torch.float32, device=dev)
+            ptr = lambda t: C.c_void_p(t.data_ptr() if t.numel() else None)
+            _abi.check(self._lib.gx_denoise_topk_edges(self._h, _abi.GX_DEVICE, C.c_void_p(em.data_ptr()), int(threshold_num), cap,
+                                                       ptr(thr), ptr(cnt), ptr(uv), ptr(vals)))
+            return thr, cnt, uv, vals
+        thr = np.zeros(count, np.float32); cnt = np.zeros(count, np.int32)
+        uv = np.zeros((count, cap, 2), np.int32); vals = np.zeros((count, cap), np.float32)
+        _abi.check(self._lib.gx_denoise_topk_edges(self._h, _abi.GX_HOST, _np_ptr(_f32c(edge_mask)), int(threshold_num), cap,
+                                                   _np_ptr(thr), _np_ptr(cnt), _np_ptr(uv), _np_ptr(vals)))
+        return thr, cnt, uv, vals
+
     def densify_host(self, edge_mask, total_dense):
         out = np.empty(total_dense, np.float64)
         _abi.check(self._lib.gx_densify(self._h, _abi.GX_HOST, _np_ptr(_f32c(edge_mask)), _np_ptr(out)))

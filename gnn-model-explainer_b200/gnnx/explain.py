@@ -132,14 +132,22 @@ class Explainer:
         self._wide_layers = self._max_width > 32
         self._no_trace = (bn or num_layers != 3 or self._wide_layers or getattr(args, "opt", "adam") != "adam" or self._att
                           or self._wide or self._head)
-        adj_np = np.asarray(adj)
+        # node mode also takes a scipy.sparse (N,N) adjacency, a batch of one graph (feat / label / pred keep their (1,N,..) shapes): a
+        # graph of 10^5 nodes has 10^10 dense entries, its CSR comes straight from the sparse matrix
+        self._sparse = _gu.is_sparse(adj)
         if graph_mode:
             # graph classification: the whole padded batch goes to the device once (explain.py:80-85)
+            if self._sparse:
+                raise ValueError("graph mode expects a dense adj of shape (G,n,n), not a sparse matrix")
+            adj_np = np.asarray(adj)
             if adj_np.ndim != 3:
                 raise ValueError("graph mode expects adj of shape (G,n,n)")
             self.engine.set_graph_batch(adj_np, np.asarray(feat), np.asarray(label))
             return
-        if adj_np.ndim != 3:
+        if self._sparse:
+            if len(adj.shape) != 2 or adj.shape[0] != adj.shape[1]:
+                raise ValueError("a sparse adj must be one (N,N) graph")
+        elif np.asarray(adj).ndim != 3:
             raise ValueError("node mode expects adj of shape (B,N,N)")
         # node tasks on a batch of graphs (explain.py:80-95 index adj / feat / label / pred with graph_idx): the engine holds one graph
         # at a time, graph 0 is uploaded now, another one when a call names it
@@ -152,11 +160,10 @@ class Explainer:
         g = 0 if graph_idx in (-1, None, False) else int(graph_idx)
         if g == self._current_graph:
             return g
-        adj_np = np.asarray(self.adj)
-        if not 0 <= g < adj_np.shape[0]:
-            raise IndexError("graph_idx %d out of range for adj of shape %s" % (g, adj_np.shape))
+        if not 0 <= g < self._num_graphs():
+            raise IndexError("graph_idx %d out of range for adj of shape %s" % (g, self.adj.shape if self._sparse else np.asarray(self.adj).shape))
         if g not in self._csr_cache:
-            self._csr_cache[g] = _gu.csr_from_dense(adj_np[g])
+            self._csr_cache[g] = _gu.csr_from_sparse(self.adj) if self._sparse else _gu.csr_from_dense(np.asarray(self.adj)[g])
         self._rowptr, self._col = self._csr_cache[g]
         feat_np = np.asarray(self.feat, dtype=np.float32)[g]
         label_np = np.asarray(self.label)[g].astype(np.int32)
@@ -174,6 +181,9 @@ class Explainer:
         self._current_graph = g
         return g
 
+    def _num_graphs(self):
+        return 1 if self._sparse else np.asarray(self.adj).shape[0]
+
     # the reference computes this dense (B,N,N) matrix eagerly in __init__ (explain.py:67); here
     # it is materialised on demand only (the engine never needs it).
     @property
@@ -181,7 +191,7 @@ class Explainer:
         if self._neighborhoods is None:
             keep = self._current_graph
             mats = []
-            for g in range(np.asarray(self.adj).shape[0]):
+            for g in range(self._num_graphs()):
                 self._select_graph(g)
                 N = self.engine.num_nodes
                 mats.append(self.engine.neighborhood_rows(np.arange(N, dtype=np.int32), self.n_hops).astype(int))
@@ -196,7 +206,10 @@ class Explainer:
         nbrs = plan.neighbors_of(0).astype(np.int64)
         # the caller's own adjacency rows / columns, exactly like the reference (adj[g][nbrs][:, nbrs]): self loops, if any, stay in
         # sub_adj (the plan's edge list drops them, as the explainer's diag_mask does for the optimisation)
-        sub_adj = np.asarray(self.adj)[graph_idx][nbrs][:, nbrs]
+        if self._sparse:
+            sub_adj = self.adj.tocsr()[nbrs][:, nbrs].toarray()
+        else:
+            sub_adj = np.asarray(self.adj)[graph_idx][nbrs][:, nbrs]
         sub_feat = np.asarray(self.feat)[graph_idx, nbrs]
         sub_label = np.asarray(self.label)[graph_idx][nbrs]
         return int(plan.node_idx_new[0]), sub_adj, sub_feat, sub_label, nbrs
@@ -585,6 +598,104 @@ class Explainer:
         """Same computation, returning (plan, edge_mask) without densifying: edge_mask[edge_off[t]:
         edge_off[t+1]] are the masked_adj entries of node t at plan.csr_of(t) (row-major order)."""
         return self._explain_batch(node_indices, graph_idx)
+
+    def explain_nodes_topk(self, node_indices, threshold_num=20, chunk_size=None, graph_idx=0):
+        """explain_nodes followed by denoise_graph's thresholding (threshold_num=20: what explain_nodes_gnn_stats and the node loop
+        of explain.py:244,308 keep of every mask), for lists whose masks do not fit on the host or the device at once (BASELINE
+        configs[4]: ~0.4 GB of plan and optimiser state per node).  The list is explained `chunk_size` nodes at a time (default: the
+        device's SM count, one task per SM) and every chunk's masks are thresholded on device (gx_denoise_topk_edges); only the kept
+        counts come back to the host.  Returns, in input order:
+          thr     float32 CUDA tensor [count]: the threshold of each node (+inf for a mask without a positive value)
+          offsets int64 numpy array [count+1]: node t's edges are rows offsets[t]:offsets[t+1] of uv / vals
+          uv      int32 CUDA tensor [total, 2]: the kept undirected edges in global node ids, u < v, ascending per node
+          vals    float32 CUDA tensor [total]: their mask values
+        A node's masks do not depend on the chunk it is explained in, so the result is the same bits for every chunk_size
+        (args.gnnx_latency is switched off for the call).  With args.gnnx_init="torch" every node draws its n^2 normals in list order:
+        M0 and torch's RNG afterwards are those of explain_nodes(node_indices).  No per-epoch trace, no .npy files."""
+        if self.graph_mode:
+            raise ValueError("explain_nodes_topk is node mode only (graph mode gathers its packed masks: gnnx.dist.explain_graphs_sharded)")
+        self._select_graph(graph_idx)
+        nodes = np.asarray(node_indices, np.int64).reshape(-1)
+        thr, cnt, uv, vals = self._topk_chunks(nodes, np.arange(len(nodes)), None, threshold_num, chunk_size)
+        return thr, np.concatenate([[0], np.cumsum(cnt)]).astype(np.int64), uv, vals
+
+    def _topk_chunks(self, nodes, positions, n_all, threshold_num, chunk_size, timings=None):
+        """The chunk loop of explain_nodes_topk over the list entries `positions` (ascending) of `nodes`.  With the torch init it makes
+        one forward walk over the list up to the last position, drawing every entry's n^2 normals and keeping those of the positions
+        explained here (n_all[p] = k-hop size of entry p, gx_count_nodes; needed for the entries not explained here), then finishes
+        the walk to the end of the list: torch's RNG ends where explain_nodes(nodes) leaves it.
+        Returns (thr CUDA [k], counts int64 numpy [k], uv CUDA [total, 2], vals CUDA [total]) of those positions.
+        timings (dict or None): accumulates the wall seconds of the phases (plan, m0, explain, topk; synchronising after each) and the
+        explainer kernels' device seconds (explain_device)."""
+        import time
+        eng = self.engine
+        dev = torch.device("cuda", eng.device)
+        if chunk_size is None:
+            chunk_size = torch.cuda.get_device_properties(dev).multi_processor_count
+        chunk_size = int(chunk_size)
+        if chunk_size < 1:
+            raise ValueError("chunk_size must be >= 1")
+        if int(threshold_num) < 1:
+            raise ValueError("threshold_num must be >= 1")
+        hp, init = self._hparams()
+        gain = torch.nn.init.calculate_gain("relu")
+        clock = [time.perf_counter()]
+
+        def tick(key):
+            if timings is not None:
+                torch.cuda.synchronize(dev)
+                now = time.perf_counter()
+                timings[key] = timings.get(key, 0.0) + now - clock[0]
+                clock[0] = now
+
+        thr_p, cnt_p, uv_p, val_p = [], [], [], []
+        walk = 0          # first list entry whose normals have not been drawn
+        latency = bool(getattr(self.args, "gnnx_latency", False))
+        if latency:
+            eng.debug_cluster(1, 0)
+        try:
+            for c0 in range(0, len(positions), chunk_size):
+                pos = np.asarray(positions[c0:c0 + chunk_size], np.int64)
+                clock[0] = time.perf_counter()
+                plan = eng.plan_nodes(nodes[pos], self.n_hops, fetch=(init == "torch"))
+                tick("plan")
+                m0_dev = None
+                if init == "torch":
+                    m0 = np.empty(plan.total_edges, dtype=np.float32)
+                    flat = plan.flat_index()
+                    eo = plan.edge_off
+                    mine = {int(p): t for t, p in enumerate(pos)}
+                    for p in range(walk, int(pos[-1]) + 1):
+                        t = mine.get(p)
+                        n = plan.n(t) if t is not None else int(n_all[p])
+                        M = torch.FloatTensor(n, n).normal_(1.0, gain * math.sqrt(2.0 / (n + n)))
+                        if t is not None:
+                            np.take(M.numpy().reshape(-1), flat[eo[t]:eo[t + 1]], out=m0[eo[t]:eo[t + 1]])
+                    walk = int(pos[-1]) + 1
+                    m0_dev = torch.from_numpy(m0).to(dev)
+                    tick("m0")
+                mask = eng.explain_nodes_device(hp, m0_dev)
+                if timings is not None:
+                    tick("explain")
+                    timings["explain_device"] = timings.get("explain_device", 0.0) + eng.last_explain_ms() / 1e3
+                thr, cnt, uv, vals = eng.denoise_topk_edges(mask, threshold_num)
+                cnt_h = cnt.cpu().numpy().astype(np.int64)
+                if int(cnt_h.max(initial=0)) > uv.shape[1]:      # values tie at the threshold: again with room for all of them
+                    thr, cnt, uv, vals = eng.denoise_topk_edges(mask, threshold_num, cap=int(cnt_h.max()))
+                keep = torch.arange(uv.shape[1], device=dev)[None, :] < cnt[:, None]
+                thr_p.append(thr); cnt_p.append(cnt_h); uv_p.append(uv[keep]); val_p.append(vals[keep])
+                tick("topk")
+        finally:
+            if latency:
+                eng.debug_cluster(0, 0)
+        if init == "torch":      # the rest of the list, so that torch's RNG ends as after one process's explain_nodes
+            for p in range(walk, len(nodes)):
+                n = int(n_all[p])
+                torch.FloatTensor(n, n).normal_(1.0, gain * math.sqrt(2.0 / (n + n)))
+        if not thr_p:
+            return (torch.zeros(0, dtype=torch.float32, device=dev), np.zeros(0, np.int64),
+                    torch.zeros((0, 2), dtype=torch.int32, device=dev), torch.zeros(0, dtype=torch.float32, device=dev))
+        return torch.cat(thr_p), np.concatenate(cnt_p), torch.cat(uv_p), torch.cat(val_p)
 
     def iter_explain_nodes_packed(self, node_indices, chunk_size, graph_idx=0, model="exp"):
         """Large graphs (BASELINE configs[4]: a k-hop neighbourhood is most of a 10^5-node graph, ~0.4 GB of plan and optimiser

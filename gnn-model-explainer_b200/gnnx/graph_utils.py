@@ -20,6 +20,29 @@ def csr_from_dense(adj):
     return np.cumsum(rowptr).astype(np.int32), ej.astype(np.int32)
 
 
+def is_sparse(adj):
+    """True for a scipy.sparse matrix (scipy is only imported when it is installed)."""
+    try:
+        import scipy.sparse as sp
+    except ImportError:
+        return False
+    return sp.issparse(adj)
+
+
+def csr_from_sparse(adj):
+    """scipy.sparse (N,N) 0/1 adjacency -> the (rowptr, col) csr_from_dense returns for adj.toarray(), without materialising the
+    dense matrix: duplicates summed, explicit zeros dropped, columns ascending per row.  Host marshalling only."""
+    if adj.ndim != 2 or adj.shape[0] != adj.shape[1]:
+        raise ValueError("adjacency must be square")
+    a = adj.tocsr(copy=True)
+    a.sum_duplicates()
+    a.eliminate_zeros()
+    a.sort_indices()
+    if a.nnz and not np.all(a.data == 1):
+        raise NotImplementedError("weighted adjacency is not built (reference datasets are 0/1)")
+    return a.indptr.astype(np.int32), a.indices.astype(np.int32)
+
+
 def neighborhoods(adj, n_hops, use_cuda=True):
     """utils/graph_utils.py:147-158: (B,N,N) 0/1 -> (B,N,N) int, (A + A^2 + ... + A^k) > 0.
 

@@ -288,6 +288,17 @@ int gx_densify(gx_handle* h, gx_memspace space, const float* edge_mask, double* 
  * This is also what a multi-GPU run gathers when the full masks are too large to gather (BASELINE configs[4]). */
 int gx_denoise_topk(gx_handle* h, gx_memspace space, const float* edge_mask, int32_t threshold_num, int32_t cap,
                     float* out_threshold, int32_t* out_count, int32_t* out_slots, float* out_vals);
+/* The same thresholding, delivered as undirected edges in GLOBAL node ids (what a multi-GPU run gathers: the records can be read
+ * without the plan that produced them).  After gx_plan_nodes (gx_plan_fetch is not needed).  Per node
+ *   out_threshold[t] = exactly gx_denoise_topk's threshold (+inf if no positive value)
+ *   out_count[t]     = number of kept slots with row < col: half of gx_denoise_topk's count for the masks the explainer kernels
+ *                      write (both directions of an edge carry the same bits); it may exceed cap when values tie
+ *   out_uv[(t*cap + i)*2 ..] = (nbrs[row], nbrs[col]) of the i-th such slot in canonical (row-major) slot order, i.e. ascending
+ *                      (u, v) with u < v; first `cap` pairs, the rest (-1, -1)
+ *   out_vals[t*cap + i]      = its mask value, 0 past the written pairs (may be NULL)
+ * All buffers in `space`. */
+int gx_denoise_topk_edges(gx_handle* h, gx_memspace space, const float* edge_mask, int32_t threshold_num, int32_t cap,
+                          float* out_threshold, int32_t* out_count, int32_t* out_uv, float* out_vals);
 
 /* ---- multi-GPU: one process per GPU, explained nodes dealt across ranks, ONE all-gather of the packed masks (SURVEY 8e) ----
  * The reference's node loop (explain.py:225-236) is sequential and has no exchange step; results of different nodes never

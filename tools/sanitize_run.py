@@ -3,7 +3,8 @@
     compute-sanitizer --tool racecheck python tools/sanitize_run.py
 k-hop extraction + shared-memory kernel on a mix of task sizes (syn1: hub node 0 and tiny tasks), the streaming kernel (forced),
 the gradient baseline, graph mode, densify, the off-edge regulariser sums of graph mode, neighbourhood rows, the unconstrained (dense) kernel, attention models, inputs wider than 128
-features (explain_var.cu's wide path), models with 5 to 7 layers, graph-mode sharding's densify (dist_graphs).  A few epochs each."""
+features (explain_var.cu's wide path), models with 5 to 7 layers, graph-mode sharding's densify (dist_graphs), top-k delivery in global ids
+(topk: gx_denoise_topk_edges with host and device buffers, and one Explainer.explain_nodes_topk call).  A few epochs each."""
 import os
 import sys
 
@@ -20,7 +21,7 @@ EPOCHS = int(os.environ.get("SAN_EPOCHS", "4"))
 
 
 def main():
-    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster", "dense", "att", "wide", "dist_graphs"]
+    which = sys.argv[1:] or ["node", "stream", "graph", "misc", "var", "cluster", "dense", "att", "wide", "dist_graphs", "topk"]
     fx = util.load_fixture("syn1")
     if "node" in which:
         eng = util.make_engine(fx)
@@ -318,6 +319,34 @@ def main():
             dense = eng.densify_graphs_host(gids, out)
             print("dist_graphs ok", n, int(e.sum()), float(dense.sum()))
             eng.close()
+    if "topk" in which:   # denoise.cu's edges mode: kernel masks, ties, a node without a positive value, a cap below the kept count;
+        # then the chunk loop of explain_nodes_topk (chunks of 3, the hub node among them)
+        import types
+        import torch
+        eng = util.make_engine(fx)
+        plan = eng.plan_nodes([0, 3, 300, 683, 13], 3)
+        out = np.zeros(plan.total_edges, np.float32)
+        eng.explain_nodes_host(eng.make_hparams(num_epochs=EPOCHS, init=_abi.GX_INIT_PHILOX, seed=3), None, out)
+        out[plan.edge_off[1]:plan.edge_off[2]] = np.round(out[plan.edge_off[1]:plan.edge_off[2]] * 4) / 4
+        out[plan.edge_off[4]:plan.edge_off[5]] = 0.0
+        thr, cnt, uv, vals = eng.denoise_topk_edges(out, 20)
+        thr_d, cnt_d, uv_d, vals_d = eng.denoise_topk_edges(torch.from_numpy(out).cuda(), 3, cap=2)
+        torch.cuda.synchronize()
+        print("topk ok edges", int(cnt.sum()), int(uv.max()), int(cnt_d.sum()))
+        eng.close()
+        import gnnx_oracle as O
+        args = types.SimpleNamespace(num_gc_layers=3, num_epochs=EPOCHS, lr=0.1, opt="adam", opt_scheduler="none", mask_act="sigmoid",
+                                     mask_bias=False, gpu=False, bias=True, method="base", dataset="syn1", bmname=None, hidden_dim=20,
+                                     output_dim=20, name_suffix="", explainer_suffix="", logdir="/tmp", gnnx_init="device", gnnx_seed=2)
+        model = gnnx.models.GcnEncoderNode(fx.feat.shape[1], 20, 20, fx.weights["Wp"].shape[0], 3, bn=False, args=args)
+        model.load_state_dict({k: torch.tensor(v) for k, v in zip(
+            ["conv_first.weight", "conv_first.bias", "conv_block.0.weight", "conv_block.0.bias", "conv_last.weight", "conv_last.bias",
+             "pred_model.weight", "pred_model.bias"], [fx.weights[k] for k in util.WKEYS])})
+        ex = gnnx.Explainer(model=model, adj=O.dense_from_csr(fx.rowptr, fx.col)[None], feat=fx.feat[None], label=fx.label[None],
+                            pred=fx.pred[None], train_idx=[], args=args, writer=None, print_training=False, graph_idx=-1)
+        thr, offsets, uv, vals = ex.explain_nodes_topk([0, 300, 5, 683, 13, 42, 7], chunk_size=3)
+        print("topk ok explain_nodes_topk", int(offsets[-1]), float(vals.sum()))
+        ex.engine.close()
 
 
 if __name__ == "__main__":
