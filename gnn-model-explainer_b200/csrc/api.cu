@@ -279,7 +279,7 @@ static int set_variant_model(gx_handle* h, const char* who, const gx_model_dims*
   h->m.Wp = b + offWp; h->m.bp = b + offbp;
   h->head = head;
   h->head.W = head.k > 0 ? b + offHead : nullptr;
-  h->has_model = true; h->has_plan = false;
+  h->has_model = true; h->has_plan = false; h->has_gplan = false;   // both plans were laid out for the previous model
   return GX_OK;
 }
 
@@ -552,6 +552,7 @@ int gx_set_model(gx_handle* h, const gx_model_dims* dims, const float* const* co
   h->head = GxHeadDev{};
   h->has_model = true;
   h->has_plan = false;
+  h->has_gplan = false;   // a graph plan's shared-memory footprints were computed for the previous model
   return GX_OK;
 }
 
@@ -735,6 +736,7 @@ int gx_denoise_topk(gx_handle* h, gx_memspace space, const float* edge_mask, int
     GX_CUDA_CHECK(stage_out(h->d_dn_vals, out_vals, nslots, &vals));
   }
   GX_CUDA_CHECK(cudaMemsetAsync(slots, 0xFF, nslots * 4, h->stream));   // unused entries read as -1
+  if (vals) GX_CUDA_CHECK(cudaMemsetAsync(vals, 0, nslots * 4, h->stream));   // and their values as 0, not a reused buffer's contents
   GX_CUDA_CHECK(gx_launch_denoise_topk(h->plan, (int)count, em, 2 * threshold_num, cap, thr, cnt, slots, vals, h->stream));
   h->launches += 1;
   if (space == GX_HOST) {

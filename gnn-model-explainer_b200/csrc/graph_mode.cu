@@ -151,6 +151,7 @@ static int explain_graphs_impl(gx_handle* h, const gx_hparams* hp, gx_memspace s
   const char* who = "gx_explain_graphs";
   if (!h || !hp) { gx_set_error("gx_explain_graphs: NULL argument"); return GX_ERR_INVALID; }
   if (!h->has_gplan) { gx_set_error("gx_explain_graphs: no plan (call gx_plan_graphs)"); return GX_ERR_INVALID; }
+  if (h->gb.d != h->m.d) { gx_set_error("gx_explain_graphs: feat_dim %d != model input_dim %d", h->gb.d, h->m.d); return GX_ERR_INVALID; }
   const bool var = h->m.variant || hp->opt != GX_OPT_ADAM;   // the whole batch through explain_var.cu
   int rc = check_explain_hparams(who, hp, 0, var, io, true);
   if (rc != GX_OK) return rc;

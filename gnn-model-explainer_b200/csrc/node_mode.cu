@@ -108,7 +108,8 @@ int gx_count_nodes(gx_handle* h, const int32_t* nodes, int32_t count, int32_t n_
   GX_CUDA_CHECK(cudaSetDevice(h->device));
   rc = ensure_slot_ws(h);
   if (rc != GX_OK) return rc;
-  h->has_plan = false;     // the task buffer is shared with the plan
+  h->has_plan = false;     // the task buffer is shared with both plans
+  h->has_gplan = false;
   GX_CUDA_CHECK(h->d_nodes.reserve((size_t)count * 4));
   GX_CUDA_CHECK(h->d_tasks.reserve((size_t)count * sizeof(GxTask)));
   GX_CUDA_CHECK(cudaMemcpyAsync(h->d_nodes.p, nodes, (size_t)count * 4, cudaMemcpyHostToDevice, h->stream));

@@ -13,6 +13,7 @@ static int explain_unconstrained_impl(gx_handle* h, bool graph, const gx_hparams
   const char* who = graph ? "gx_explain_graphs_unconstrained" : "gx_explain_nodes_unconstrained";
   if (!h || !hp || !edge_mask) { gx_set_error("%s: NULL argument", who); return GX_ERR_INVALID; }
   if (graph ? !h->has_gplan : !h->has_plan) { gx_set_error("%s: no plan (call %s)", who, graph ? "gx_plan_graphs" : "gx_plan_nodes"); return GX_ERR_INVALID; }
+  if (graph && h->gb.d != h->m.d) { gx_set_error("%s: feat_dim %d != model input_dim %d", who, h->gb.d, h->m.d); return GX_ERR_INVALID; }
   int rc = check_explain_hparams(who, hp, 0, false, nullptr, graph);
   if (rc != GX_OK) return rc;
   if (h->has_model && h->m.att) {

@@ -110,6 +110,7 @@ def explain_nodes_sharded(explainer, node_indices, costs=None, group=None, use_e
     values[offsets[t]:offsets[t+1]] are the masked_adj entries of node_indices[t] at the row-major sub-adjacency slots."""
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     eng = explainer.engine
+    eng.follow_torch_stream()
     nodes = np.asarray(node_indices)
     dev = torch.device("cuda", eng.device)
     n_all, e_all = count_nodes_cached(explainer, nodes)
@@ -151,6 +152,7 @@ def explain_graphs_sharded(explainer, graph_indices, costs=None, group=None, use
         raise ValueError("explain_graphs_sharded needs an Explainer constructed with graph_mode=True")
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     eng = explainer.engine
+    eng.follow_torch_stream()
     gids = np.asarray(graph_indices, np.int64)
     dev = torch.device("cuda", eng.device)
     key = (gids.tobytes(), world, None if costs is None else np.asarray(costs).tobytes())
@@ -197,6 +199,7 @@ def explain_nodes_topk_sharded(explainer, node_indices, threshold_num=20, chunk_
     eng = explainer.engine
     if explainer.graph_mode:
         raise ValueError("explain_nodes_topk_sharded is node mode only")
+    eng.follow_torch_stream()
     nodes = np.asarray(node_indices, np.int64).reshape(-1)
     dev = torch.device("cuda", eng.device)
     t0 = time.perf_counter()

@@ -100,6 +100,13 @@ class Engine:
     def set_stream(self, cuda_stream_ptr):
         _abi.check(self._lib.gx_set_stream(self._h, C.c_void_p(int(cuda_stream_ptr))))
 
+    def follow_torch_stream(self):
+        """Binds the engine to torch's current stream on its device: the engine's work on device tensors is then ordered with the torch
+        ops that fill or read them, and the caching allocator reuses them only after the engine is done.  The drop-in (Explainer,
+        gnnx.dist) calls this at the start of every call that hands device tensors between torch and the engine."""
+        import torch
+        self.set_stream(torch.cuda.current_stream(self.device).cuda_stream)
+
     def sync(self):
         _abi.check(self._lib.gx_sync(self._h))
 
@@ -205,6 +212,7 @@ class Engine:
         tn, te = C.c_int64(), C.c_int64()
         _abi.check(self._lib.gx_plan_nodes(self._h, _np_ptr(nodes), len(nodes), int(n_hops), C.byref(tn), C.byref(te)))
         self._plan_sizes = (len(nodes), tn.value, te.value)
+        self._plan = None
         if not fetch:
             return None
         return self.fetch_plan(nodes)
@@ -396,8 +404,10 @@ class Engine:
         return out[:total]
 
     def _dense_total(self):
-        p = self._plan
-        return int(np.sum(np.diff(p.node_off).astype(np.int64) ** 2))
+        """sum_t n_t^2 of the library's current node plan (gx_plan_fetch's node offsets: a host-side copy, no device work)."""
+        node_off = np.empty(self._plan_sizes[0] + 1, np.int64)
+        _abi.check(self._lib.gx_plan_fetch(self._h, _np_ptr(node_off), None, None, None, None, None))
+        return int(np.sum(np.diff(node_off) ** 2))
 
     # ---------------------------------------------------------------- multi-GPU (one all-gather of the masks)
     def count_nodes(self, nodes, n_hops):

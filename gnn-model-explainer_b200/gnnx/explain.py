@@ -479,6 +479,7 @@ class Explainer:
         else:
             nodes = [int(i) for i in node_indices]
             eng = self.engine
+            eng.follow_torch_stream()
             plan = eng.plan_nodes(nodes, self.n_hops)
             hp, init = self._hparams()
             dev = torch.device("cuda", eng.device)
@@ -614,6 +615,7 @@ class Explainer:
         M0 and torch's RNG afterwards are those of explain_nodes(node_indices).  No per-epoch trace, no .npy files."""
         if self.graph_mode:
             raise ValueError("explain_nodes_topk is node mode only (graph mode gathers its packed masks: gnnx.dist.explain_graphs_sharded)")
+        self.engine.follow_torch_stream()
         self._select_graph(graph_idx)
         nodes = np.asarray(node_indices, np.int64).reshape(-1)
         thr, cnt, uv, vals = self._topk_chunks(nodes, np.arange(len(nodes)), None, threshold_num, chunk_size)

@@ -14,6 +14,15 @@
  *   - One handle per host thread / per GPU.  Calls on one handle must not overlap.
  *   - All work is issued on the stream set with gx_set_stream (default: the legacy default
  *     stream); calls that return results to host memory synchronise that stream before returning.
+ *   - A handle holds one plan at a time, a node plan (gx_plan_nodes) or a graph plan (gx_plan_graphs):
+ *     each of the two calls replaces the other's plan.  Both plans are dropped by gx_set_model,
+ *     gx_set_model_att and gx_set_model_head (a plan is laid out for the model it was made under) and
+ *     by gx_count_nodes (it reuses the plan's task buffer).  The node plan is also dropped by
+ *     gx_set_graph_csr, gx_debug_set_cluster and gx_debug_force_stream; the graph plan by
+ *     gx_set_graph_batch_csr.  Every other call keeps the plan: explain calls, gx_set_stream, the
+ *     other mode's graph upload, gx_model_forward, gx_neighborhood_rows, gx_count_graphs,
+ *     gx_densify_graphs and the other debug knobs.  A call that needs a dropped plan fails with
+ *     GX_ERR_INVALID ("no plan") before it touches the device.
  *   - There is NO CPU fallback: without a CUDA device gx_create fails with GX_ERR_CUDA.
  */
 #ifndef GNNX_H_
@@ -284,7 +293,7 @@ int gx_densify(gx_handle* h, gx_memspace space, const float* edge_mask, double* 
  *   out_threshold[t] = the min(2k, #positive)-th largest positive mask value ("edges are repeated twice in adj"), +inf if none
  *   out_count[t]     = number of directed slots with value >= threshold (>= 2k when values tie at the threshold)
  *   out_slots[t*cap ..] = those slots (task-local indices into the node's sub_col / edge_mask slice), ascending, first `cap`
- *   out_vals[t*cap ..]  = their mask values (may be NULL)
+ *   out_vals[t*cap ..]  = their mask values, 0 past the written slots (may be NULL)
  * This is also what a multi-GPU run gathers when the full masks are too large to gather (BASELINE configs[4]). */
 int gx_denoise_topk(gx_handle* h, gx_memspace space, const float* edge_mask, int32_t threshold_num, int32_t cap,
                     float* out_threshold, int32_t* out_count, int32_t* out_slots, float* out_vals);
