@@ -103,6 +103,7 @@ struct GraphArgs {
   float* out_mask;
   float* out_feat;
   GxExtra x;
+  const int32_t* grad_label;   // hp.mode == 1: the loss label of every task (-1: the arg-max of the logits this forward produces)
 };
 
 template <int HID, int EMB, int NT, bool kTrace>
@@ -129,7 +130,10 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_graph_kernel(const Grap
     if (qi >= A.ntasks) break;
     const int task_id = A.order[qi];
     const GxTask* __restrict__ Tp = A.plan.tasks + task_id;
-    const int na = Tp->n, e_d = Tp->e_d, np = Tp->npairs, gt = Tp->gt_label, g = Tp->node;
+    const int na = Tp->n, e_d = Tp->e_d, np = Tp->npairs, g = Tp->node;
+    // gradient baseline: the loss is taken at the label the caller gives (the graph's predicted label, explain.py:102,129),
+    // otherwise at label[graph] (explain.py:750-753)
+    const int gt = hp.mode ? __ldg(A.grad_label + task_id) : Tp->gt_label;
     const bool has_const = (Tp->flags & 1) != 0;
     const int64_t node_off = Tp->node_off, rp_off = Tp->rp_off, edge_off = Tp->edge_off, pair_off = Tp->pair_off;
     if (tid == 0) sL = gx_make_layout_graph(na, e_d, np, d, HID, EMB, C, nwarps);
@@ -177,7 +181,8 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_graph_kernel(const Grap
     for (int i = tid; i <= na; i += nthreads) irp[i] = (IdxT)A.plan.irowptr[rp_off + i];
     const bool resume = hp.init == GX_INIT_STATE;   // optimiser state supplied by the caller (gx_explain_io)
     for (int f = tid; f < dp; f += nthreads) {
-      sF[f] = 0.5f; Fm[f] = 0.f; mF[f] = 0.f; vF[f] = 0.f;
+      sF[f] = hp.mode ? 1.0f : 0.5f;   // sigmoid(0) (explain.py:633-643); gradient baseline: unmasked features
+      Fm[f] = 0.f; mF[f] = 0.f; vF[f] = 0.f;
       if (resume && A.x.feat_state_in != nullptr && f < d) {
         const float* fs = A.x.feat_state_in + (int64_t)task_id * 3 * d;
         Fm[f] = fs[f]; mF[f] = fs[d + f]; vF[f] = fs[2 * d + f];
@@ -197,6 +202,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_graph_kernel(const Grap
       const int pij = A.plan.pair_pij[pair_off + p], pji = A.plan.pair_pji[pair_off + p];
       const int oij = A.plan.pair_oij[pair_off + p], oji = A.plan.pair_oji[pair_off + p];
       pi[p] = (IdxT)i; pj[p] = (IdxT)j; ppij[p] = (IdxT)pij; ppji[p] = (IdxT)pji;
+      if (hp.mode) { a[pij] = 1.0f; a[pji] = 1.0f; continue; }   // gradient baseline: the adjacency itself, no mask parameters
       float Mi, Mj;
       if (hp.init != GX_INIT_PHILOX) { Mi = __ldg(A.m0 + edge_off + oij); Mj = __ldg(A.m0 + edge_off + oji); }
       else {
@@ -314,6 +320,12 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_graph_kernel(const Grap
         for (int c = lane; c < C; c += 32) se += expf(logit[c] - mx);
         se = warp_sum(se);
         __syncwarp();
+        int lbl = gt;
+        if (lbl < 0) {   // gradient baseline without a label: the model's own prediction, first maximum (np.argmax)
+          lbl = 0;
+          for (int c = 1; c < C; ++c) lbl = logit[c] > logit[lbl] ? c : lbl;
+          __syncwarp();   // every lane has read the logits before they are overwritten below
+        }
         if (kTrace) {
           float* const tr = s_tr + (NT / 32) * 4;
           if (lane == 0) { const float lg = logit[gt]; tr[0] = -((lg - mx) - logf(se)); tr[1] = expf(lg - mx) / se; }
@@ -327,7 +339,7 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_graph_kernel(const Grap
           if (lane == 0) tr[2] = hp.c_feat_size * fs / (float)d;
           __syncwarp();
         }
-        for (int c = lane; c < C; c += 32) logit[c] = expf(logit[c] - mx) / se - (c == gt ? 1.f : 0.f);
+        for (int c = lane; c < C; c += 32) logit[c] = expf(logit[c] - mx) / se - (c == lbl ? 1.f : 0.f);
         __syncwarp();
         for (int k = lane; k < PD; k += 32) {
           float t = 0.f;
@@ -404,7 +416,19 @@ __global__ void __launch_bounds__(NT, 1024 / NT) explain_graph_kernel(const Grap
         __syncthreads();
       }
       // ---- edge phase: every edge sees all three layers; no Laplacian term in graph mode (explain.py:787-788)
-      {
+      if (hp.mode) {
+        // gradient baseline (explain.py:128-133): mask_ij = sigmoid(|dL/dA_ij| + |dL/dA_ji|) on both slots, no regulariser, no update
+        for (int p = tid; p < np; p += nthreads) {
+          const int i = pi[p], j = pj[p];
+          const float gij = dot_v4(U + i * dp, X + j * dp, D4) + dot_relu_v4(dZ2 + i * HS, Yh1 + j * HS, H4)
+                          + dot_relu_v4(dZ3 + i * HS, Yh2 + j * HS, H4);
+          const float gji = dot_v4(U + j * dp, X + i * dp, D4) + dot_relu_v4(dZ2 + j * HS, Yh1 + i * HS, H4)
+                          + dot_relu_v4(dZ3 + j * HS, Yh2 + i * HS, H4);
+          const float an = sigmoid_f(fabsf(gij) + fabsf(gji));
+          A.out_mask[edge_off + A.plan.pair_oij[pair_off + p]] = an;
+          A.out_mask[edge_off + A.plan.pair_oji[pair_off + p]] = an;
+        }
+      } else {
         const float2 tab = __ldg(hp.adam_tab + (it - 1));
         const float step = tab.x, bc2s = tab.y, bc2s_inv = 1.0f / tab.y;
         const bool last = (it == hp.out_iter);   // the mask built after this update is the one the reference returns
@@ -491,10 +515,10 @@ cudaError_t gx_launch_graph_plan(const GxGraphBatchDev& gb, int count, GxPlanArr
 
 cudaError_t gx_launch_explain_graphs(const GxExplainLaunch& cfg, const GxGraphBatchDev& gb, const GxModelDev& m,
                                      const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0, float* out_mask,
-                                     float* out_feat, cudaStream_t s) {
+                                     float* out_feat, const int32_t* grad_label, cudaStream_t s) {
   GraphArgs args;
   fill_queue_args(args, cfg, m, hp, plan, m0, out_mask, out_feat);
-  args.gb = gb; args.x = cfg.x;
+  args.gb = gb; args.x = cfg.x; args.grad_label = grad_label;
   const bool tr = cfg.x.trace != nullptr;
   auto launch = [&](auto kern) -> cudaError_t {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cfg.smem_bytes);

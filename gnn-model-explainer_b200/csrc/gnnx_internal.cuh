@@ -414,9 +414,10 @@ struct GxGraphBatchDev {
   const int32_t* label;   // [G]
 };
 cudaError_t gx_launch_graph_plan(const GxGraphBatchDev& gb, int count, GxPlanArrays plan, cudaStream_t s);
+// grad_label: hp.mode == 1 only, one loss label per task (-1: the forward's arg-max)
 cudaError_t gx_launch_explain_graphs(const GxExplainLaunch& cfg, const GxGraphBatchDev& gb, const GxModelDev& m,
                                      const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0, float* out_mask,
-                                     float* out_feat, cudaStream_t s);
+                                     float* out_feat, const int32_t* grad_label, cudaStream_t s);
 // explain_var.cu: the model and optimiser variants, node mode (graph_mode 0, g) or graph mode (gb)
 cudaError_t gx_launch_explain_var(const GxExplainLaunch& cfg, int graph_mode, const GxGraphDev& g, const GxGraphBatchDev& gb,
                                   const GxModelDev& m, const GxHeadDev& hd, const GxHparamsDev& hp, const GxPlanArrays& plan, const float* m0,

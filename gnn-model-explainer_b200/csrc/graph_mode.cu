@@ -1,6 +1,6 @@
 // graph_mode.cu -- graph classification on the host side of libgnnx.so: the padded graph batch, gx_plan_graphs (one task per graph,
 // sorted into launch classes by shared-memory footprint), gx_explain_graphs, and the graph-list helpers of a sharded run: gx_count_graphs
-// and gx_densify_graphs (its kernel: densify_graphs.cu).
+// and gx_densify_graphs (its kernel: densify_graphs.cu); gx_grad_graphs, the gradient baseline, on the same launch classes.
 #include <string.h>
 
 #include <algorithm>
@@ -147,25 +147,43 @@ int gx_plan_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int64_
 
 }  // extern "C"
 
-static int explain_graphs_impl(gx_handle* h, const gx_hparams* hp, gx_memspace space, const gx_explain_io* io) {
-  const char* who = "gx_explain_graphs";
-  if (!h || !hp) { gx_set_error("gx_explain_graphs: NULL argument"); return GX_ERR_INVALID; }
-  if (!h->has_gplan) { gx_set_error("gx_explain_graphs: no plan (call gx_plan_graphs)"); return GX_ERR_INVALID; }
-  if (h->gb.d != h->m.d) { gx_set_error("gx_explain_graphs: feat_dim %d != model input_dim %d", h->gb.d, h->m.d); return GX_ERR_INVALID; }
+// mode 0: Explainer.explain's optimisation loop; mode 1: its model="grad" baseline (one forward/backward, explain.py:125-133,717-738)
+// at grad_label (host, one label per planned graph in [-1, C)).
+static int explain_graphs_impl(gx_handle* h, const gx_hparams* hp, int mode, gx_memspace space, const gx_explain_io* io,
+                               const int32_t* grad_label = nullptr) {
+  const char* who = mode ? "gx_grad_graphs" : "gx_explain_graphs";
+  if (!h || !hp) { gx_set_error("%s: NULL argument", who); return GX_ERR_INVALID; }
+  if (!h->has_gplan) { gx_set_error("%s: no plan (call gx_plan_graphs)", who); return GX_ERR_INVALID; }
+  if (h->gb.d != h->m.d) { gx_set_error("%s: feat_dim %d != model input_dim %d", who, h->gb.d, h->m.d); return GX_ERR_INVALID; }
   const bool var = h->m.variant || hp->opt != GX_OPT_ADAM;   // the whole batch through explain_var.cu
-  int rc = check_explain_hparams(who, hp, 0, var, io, true);
+  int rc = check_explain_hparams(who, hp, mode, var, io, true);
   if (rc != GX_OK) return rc;
-  GX_CUDA_CHECK(cudaSetDevice(h->device));
   const int count = h->count;
+  if (mode == 1) {
+    if (!grad_label) { gx_set_error("%s: pred_label is NULL", who); return GX_ERR_INVALID; }
+    for (int t = 0; t < count; ++t)
+      if (grad_label[t] < -1 || grad_label[t] >= h->m.C) {
+        gx_set_error("%s: pred_label[%d] = %d outside [-1,%d)", who, t, grad_label[t], h->m.C);
+        return GX_ERR_INVALID;
+      }
+  }
+  GX_CUDA_CHECK(cudaSetDevice(h->device));
   const int64_t te = h->total_e;
   IoDev D;
-  rc = io_prepare(h, who, hp, 0, space, io, count, te, h->m.d, h->m.C, &D);
+  rc = io_prepare(h, who, hp, mode, space, io, count, te, h->m.d, h->m.C, &D);
   if (rc != GX_OK) return rc;
   D.x.tr_outer = nullptr;   // graph mode has no outer pairs
+  const int32_t* d_label = nullptr;
+  if (mode == 1) {
+    GX_CUDA_CHECK(h->d_glabel.reserve((size_t)count * 4));
+    // pageable source: the copy is staged before the call returns
+    GX_CUDA_CHECK(cudaMemcpyAsync(h->d_glabel.p, grad_label, (size_t)count * 4, cudaMemcpyHostToDevice, h->stream));
+    d_label = h->d_glabel.as<int32_t>();
+  }
   GxHparamsDev hd;
-  fill_hparams(h, hp, 0, D.x.trace != nullptr, &hd);
+  fill_hparams(h, hp, mode, D.x.trace != nullptr, &hd);
   hd.c_lap = 0.f;           // lap_loss = 0 in graph mode (explain.py:787-788)
-  rc = upload_adam_table(h, hp, hd.iters, hp->start_step);
+  rc = upload_adam_table(h, hp, hd.iters, mode == 0 ? hp->start_step : 0);
   if (rc != GX_OK) return rc;
   hd.adam_tab = h->d_adam.as<float2>();
   GX_CUDA_CHECK(cudaMemsetAsync(h->d_counters.p, 0, kNumClasses * 4, h->stream));
@@ -186,7 +204,9 @@ static int explain_graphs_impl(gx_handle* h, const gx_hparams* hp, gx_memspace s
       cfg[c].x = D.x;
       slabs[c] = cfg[c].grid;
     }
-    auto launch = [&](int, const GxExplainLaunch& k, cudaStream_t s) { return gx_launch_explain_graphs(k, h->gb, h->m, hd, h->plan, D.m0, D.out, D.feat, s); };
+    auto launch = [&](int, const GxExplainLaunch& k, cudaStream_t s) {
+      return gx_launch_explain_graphs(k, h->gb, h->m, hd, h->plan, D.m0, D.out, D.feat, d_label, s);
+    };
     rc = launch_classes(h, kNumGraphClasses, cfg, slabs, launch, [] { return (int)GX_OK; });
     if (rc != GX_OK) return rc;
   }
@@ -206,11 +226,20 @@ int gx_explain_graphs(gx_handle* h, const gx_hparams* hp, gx_memspace space, con
   gx_explain_io io;
   memset(&io, 0, sizeof(io));
   io.m0_edges = m0_edges; io.edge_mask = edge_mask; io.feat_mask = feat_mask;
-  return explain_graphs_impl(h, hp, space, &io);
+  return explain_graphs_impl(h, hp, 0, space, &io);
 }
 
 int gx_explain_graphs_ex(gx_handle* h, const gx_hparams* hp, gx_memspace space, const gx_explain_io* io) {
-  return explain_graphs_impl(h, hp, space, io);
+  return explain_graphs_impl(h, hp, 0, space, io);
+}
+
+int gx_grad_graphs(gx_handle* h, gx_memspace space, const int32_t* pred_label, float* edge_mask) {
+  gx_hparams hp;
+  gx_default_hparams(&hp);
+  gx_explain_io io;
+  memset(&io, 0, sizeof(io));
+  io.edge_mask = edge_mask;
+  return explain_graphs_impl(h, &hp, 1, space, &io, pred_label);
 }
 
 int gx_count_graphs(gx_handle* h, const int32_t* graph_ids, int32_t count, int32_t* n_out, int32_t* e_out) {

@@ -112,6 +112,7 @@ struct gx_handle {
   GxGraphBatchDev gb{};
   DevBuf gb_rowptr, gb_col, gb_feat, gb_label;
   DevBuf d_dgraph;   // gx_densify_graphs: the value offsets and ids of its list
+  DevBuf d_glabel;   // gx_grad_graphs: the loss label of every planned graph
   std::vector<int32_t> gb_h_rowptr, gb_h_label;
   // slot workspace
   DevBuf ws_buf;

@@ -21,7 +21,7 @@ EXPORTS = [
     "gx_default_hparams", "gx_last_error", "gx_version", "gx_create", "gx_destroy", "gx_set_stream",
     "gx_sync", "gx_set_model", "gx_set_graph_csr", "gx_neighborhood_rows", "gx_plan_nodes",
     "gx_plan_fetch", "gx_explain_nodes", "gx_densify", "gx_launch_count", "gx_last_explain_ms",
-    "gx_set_graph_batch_csr", "gx_plan_graphs", "gx_explain_graphs", "gx_grad_nodes",
+    "gx_set_graph_batch_csr", "gx_plan_graphs", "gx_explain_graphs", "gx_grad_nodes", "gx_grad_graphs",
     "gx_explain_nodes_ex", "gx_explain_graphs_ex", "gx_offedge_regularisers", "gx_offedge_regularisers_graphs",
     "gx_debug_force_stream", "gx_debug_ieee_edge", "gx_debug_set_dump", "gx_debug_set_gang", "gx_debug_set_cluster", "gx_denoise_topk",
     "gx_model_forward", "gx_comm_unique_id", "gx_comm_init", "gx_comm_destroy", "gx_count_nodes", "gx_allgather_masks", "gx_unshard_masks",
@@ -102,6 +102,7 @@ def lib():
     L.gx_offedge_regularisers.argtypes = [vp, C.POINTER(GxHparams), C.c_int, f32p, vp]
     L.gx_offedge_regularisers_graphs.argtypes = [vp, C.POINTER(GxHparams), C.c_int, f32p, vp]
     L.gx_grad_nodes.argtypes = [vp, C.c_int, f32p]
+    L.gx_grad_graphs.argtypes = [vp, C.c_int, i32p, f32p]
     L.gx_denoise_topk.argtypes = [vp, C.c_int, f32p, C.c_int32, C.c_int32, f32p, i32p, i32p, f32p]
     L.gx_denoise_topk_edges.argtypes = [vp, C.c_int, f32p, C.c_int32, C.c_int32, f32p, i32p, i32p, f32p]
     L.gx_comm_unique_id.argtypes = [C.c_char_p]

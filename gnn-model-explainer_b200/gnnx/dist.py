@@ -138,7 +138,7 @@ def explain_nodes_sharded(explainer, node_indices, costs=None, group=None, use_e
     return values, offsets, (plan, pos)
 
 
-def explain_graphs_sharded(explainer, graph_indices, costs=None, group=None, use_engine_comm=True, dense=False):
+def explain_graphs_sharded(explainer, graph_indices, costs=None, group=None, use_engine_comm=True, dense=False, model="exp"):
     """Explainer(graph_mode=True).explain_graphs across all ranks of the default process group (or `group`): each rank explains its
     share of the graph list, ONE all-gather delivers every graph's packed masks.  Every model and optimiser explain_graphs accepts.
     costs: per-graph cost for the balance (default: the graph's directed edges, gx_count_graphs).  The layout is remembered for the list
@@ -147,9 +147,14 @@ def explain_graphs_sharded(explainer, graph_indices, costs=None, group=None, use
     values[offsets[t]:offsets[t+1]] are the masked_adj entries of graph_indices[t] at its CSR slots (row-major).  dense=True appends the
     (len(graph_indices), max_nodes, max_nodes) float64 CUDA tensor of the dense arrays explain_graphs returns (gx_densify_graphs).
     With args.gnnx_init = "torch" every rank draws the n^2 normals of EVERY graph of the list (torch's RNG ends as after one process's
-    explain_graphs); "device" draws nothing on the host.  Unlike explain_graphs it prints no per-epoch trace and writes no .npy files."""
+    explain_graphs); "device" draws nothing on the host.  Unlike explain_graphs it prints no per-epoch trace and writes no .npy files.
+    model="grad": the gradient baseline of every graph (explain_graphs(model="grad")), dealt, gathered and densified the same way."""
     if not explainer.graph_mode:
         raise ValueError("explain_graphs_sharded needs an Explainer constructed with graph_mode=True")
+    if model not in ("exp", "grad"):
+        raise NotImplementedError("model=%r is not built in graph mode" % model)
+    if model == "grad":
+        explainer._check_graph_grad()     # before any RNG is consumed
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     eng = explainer.engine
     eng.follow_torch_stream()
@@ -169,7 +174,10 @@ def explain_graphs_sharded(explainer, graph_indices, costs=None, group=None, use
         m0_host = explainer._draw_graph_m0_subset(eng.batch_n, len(gids), pos, [eng.graph_rows_cols(int(g)) for g in gids[pos]])
     if len(pos):
         edge_off = eng.plan_graphs(gids[pos])
-        local = eng.explain_graphs_device(hp, None if m0_host is None else torch.from_numpy(m0_host).to(dev))
+        if model == "grad":
+            local = eng.grad_graphs_device(explainer._graph_grad_labels(gids[pos]))
+        else:
+            local = eng.explain_graphs_device(hp, None if m0_host is None else torch.from_numpy(m0_host).to(dev))
     else:
         edge_off, local = None, torch.zeros(0, dtype=torch.float32, device=dev)
     if use_engine_comm:

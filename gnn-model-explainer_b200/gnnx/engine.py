@@ -378,6 +378,29 @@ class Engine:
         """Gradient baseline (explain(model="grad")) of every planned node into a host buffer."""
         _abi.check(self._lib.gx_grad_nodes(self._h, _abi.GX_HOST, _np_ptr(edge_mask_out)))
 
+    def _graph_labels(self, pred_label):
+        lbl = _i32c(pred_label).reshape(-1)
+        if lbl.size != self._graph_count:
+            raise ValueError("pred_label has %d entries for %d planned graphs" % (lbl.size, self._graph_count))
+        return lbl
+
+    def grad_graphs_host(self, pred_label, edge_mask_out):
+        """Gradient baseline (explain(..., graph_mode=True, model="grad")) of every planned graph into a host buffer (gx_grad_graphs).
+        pred_label: the loss label of every planned graph in plan order, -1 = the model's own prediction."""
+        lbl = self._graph_labels(pred_label)
+        _abi.check(self._lib.gx_grad_graphs(self._h, _abi.GX_HOST, _np_ptr(lbl), _np_ptr(edge_mask_out)))
+
+    def grad_graphs_device(self, pred_label, out=None):
+        """The same into DEVICE memory: -> torch.float32 CUDA tensor [total_edges]; asynchronous on the engine's stream (pred_label is
+        a host array)."""
+        import torch
+        lbl = self._graph_labels(pred_label)
+        te = self._graph_total
+        if out is None:
+            out = torch.empty(max(te, 1), dtype=torch.float32, device=torch.device("cuda", self.device))
+        _abi.check(self._lib.gx_grad_graphs(self._h, _abi.GX_DEVICE, _np_ptr(lbl), C.c_void_p(out.data_ptr())))
+        return out[:te]
+
     def explain_nodes_ptr(self, hp, space, m0_ptr, out_ptr, feat_ptr=0):
         _abi.check(self._lib.gx_explain_nodes(self._h, C.byref(hp), int(space), C.c_void_p(int(m0_ptr) or None),
                                               C.c_void_p(int(out_ptr)), C.c_void_p(int(feat_ptr) or None)))

@@ -132,6 +132,9 @@ class Explainer:
         self._wide_layers = self._max_width > 32
         self._no_trace = (bn or num_layers != 3 or self._wide_layers or getattr(args, "opt", "adam") != "adam" or self._att
                           or self._wide or self._head)
+        # the models the tuned kernels run (the gradient baseline's coverage): 3 layers, widths <= 32, no --bn / attention / head,
+        # inputs up to 128 features
+        self._variant = bn or num_layers != 3 or self._wide_layers or self._att or self._wide or self._head
         # node mode also takes a scipy.sparse (N,N) adjacency, a batch of one graph (feat / label / pred keep their (1,N,..) shapes): a
         # graph of 10^5 nodes has 10^10 dense entries, its CSR comes straight from the sparse matrix
         self._sparse = _gu.is_sparse(adj)
@@ -427,6 +430,10 @@ class Explainer:
             if not unconstrained and dense is not None:   # the unconstrained kernel's loss already covers all n^2 entries
                 off = self.engine.offedge_regularisers_graphs(hp, dense)
             self.last_trace = self._print_trace(hp, trace, pred, off, np.full(len(gids), float(n) * n))
+        return self._dense_graphs(rc, edge_off, edge_mask)
+
+    def _dense_graphs(self, rc, edge_off, edge_mask):
+        n = self.engine.batch_n
         out = []
         for t, (rows, cols) in enumerate(rc):
             D = np.zeros((n, n), dtype=np.float64)
@@ -434,12 +441,46 @@ class Explainer:
             out.append(D)
         return out
 
-    def explain_graphs(self, graph_indices, save=True):
+    def _check_graph_grad(self):
+        if self._variant:
+            raise NotImplementedError("model='grad' in graph mode is built for the default model only (3 layers, hidden and output "
+                                      "widths <= 32, no --bn, attention or MLP head, inputs <= 128 features)")
+
+    def _graph_grad_labels(self, gids):
+        """The loss label of model="grad" for every graph of `gids`: argmax(pred[0][g]) (explain.py:102), or -1 (the model's own
+        prediction, arg-max of the logits of gx_grad_graphs' forward) when the Explainer has no stored predictions."""
+        if self.pred is None:
+            return np.full(len(gids), -1, np.int32)
+        return np.argmax(np.asarray(self.pred)[0][np.asarray(gids, np.int64)], axis=-1).astype(np.int32)
+
+    def _graph_grad_batch(self, graph_indices):
+        """explain.py:97-133 in graph mode with model="grad" for a list of graphs, one launch (gx_grad_graphs): the gradient of
+        -log softmax(logits)[label] with respect to the unmasked padded adjacency, sigmoid(|g| + |g|^T) * adj.  unconstrained is
+        ignored, as in the reference."""
+        self._check_graph_grad()          # before any RNG is consumed
+        gids = [int(g) for g in graph_indices]
+        edge_off = self.engine.plan_graphs(gids)
+        labels = self._graph_grad_labels(gids)
+        if self._hparams()[1] == "torch":
+            # the reference still constructs an ExplainModule per graph, i.e. draws its n^2 normals (explain.py:645-652): keep the RNG in step
+            self._draw_graph_m0_subset(self.engine.batch_n, len(gids), [], [])
+        edge_mask = np.empty(max(int(edge_off[-1]), 1), dtype=np.float32)
+        try:
+            self.engine.grad_graphs_host(labels, edge_mask)
+        except _abi.GnnxError as e:
+            if e.status == _abi.GX_ERR_UNSUPPORTED:
+                raise NotImplementedError(str(e)) from None
+            raise
+        return self._dense_graphs([self.engine.graph_rows_cols(g) for g in gids], edge_off, edge_mask)
+
+    def explain_graphs(self, graph_indices, save=True, model="exp"):
         """explain.py:356-402 -> list of (n,n) masked adjacencies (one batched launch; the reference's
-        denoise_graph/log_graph drawing is out of scope)."""
+        denoise_graph/log_graph drawing is out of scope).  model="grad": the gradient baseline of every graph instead (explain.py:125-133)."""
         if not self.graph_mode:
             raise ValueError("Explainer was not constructed with graph_mode=True")
-        out = self._explain_graph_batch(graph_indices)
+        if model not in ("exp", "grad"):
+            raise NotImplementedError("model=%r is not built in graph mode" % model)
+        out = self._graph_grad_batch(graph_indices) if model == "grad" else self._explain_graph_batch(graph_indices)
         if save:
             for m in out:
                 self._save(m, 0)      # the reference overwrites one file: node_idx_0 graph_idx_<self.graph_idx>
@@ -451,9 +492,12 @@ class Explainer:
         if graph_mode or self.graph_mode:
             if not self.graph_mode:
                 raise ValueError("Explainer was not constructed with graph_mode=True")
-            if model != "exp":
-                raise NotImplementedError("only model='exp' is built in graph mode")
-            masked_adj = self._explain_graph_batch([graph_idx], unconstrained)[0]
+            if model not in ("exp", "grad"):
+                raise NotImplementedError("model=%r is not built in graph mode" % model)
+            if model == "grad":
+                masked_adj = self._graph_grad_batch([graph_idx])[0]
+            else:
+                masked_adj = self._explain_graph_batch([graph_idx], unconstrained)[0]
             fname = self._save(masked_adj, node_idx)
             if self.print_training:
                 print("Saved adjacency matrix to ", fname)

@@ -242,6 +242,18 @@ int gx_offedge_regularisers_graphs(gx_handle* h, const gx_hparams* hp, gx_memspa
  * GX_ERR_UNSUPPORTED (the message names the node) when some planned neighbourhood contains a node with a self loop: the
  * reference differentiates its raw sub_adj, diagonal included, and returns a diagonal entry the sub_col slots have no room for. */
 int gx_grad_nodes(gx_handle* h, gx_memspace space, float* edge_mask);
+/* The same baseline in graph-classification mode, Explainer.explain(0, graph_idx=g, graph_mode=True, model="grad")
+ * (explain.py:102,128-133 with adj_feat_grad's graph branch, :717-738), for every graph of gx_plan_graphs: one forward of the frozen
+ * model on the unmasked padded graph and features, loss = -log softmax(logits)[pred_label[t]], one backward to the adjacency;
+ *   pred_label [count] int32, HOST memory whatever `space` is: the loss label of planned graph t in plan order, in [-1, C); -1 = the
+ *              model's own prediction, the arg-max of the logits this forward computes (first maximum, as np.argmax) -- what the
+ *              reference's argmax(pred[0][g]) is when pred holds the model's output.  The graph's label is not used;
+ *   edge_mask  [total_edges] float32 in `space`: sigmoid(|dL/dA_ij| + |dL/dA_ji|) at the graph's CSR slots (what the reference
+ *              returns at its adjacency entries, batch index 0).
+ * The reference's explain() itself cannot run this path (it indexes the scalar label, explain.py:129); its adj_feat_grad can, and
+ * this is its result.  Default model only (3 layers, widths <= 32, no --bn / attention / head, d <= 128): GX_ERR_UNSUPPORTED for
+ * model variants, as gx_grad_nodes; GX_ERR_INVALID for a label outside [-1, C) or without a graph plan. */
+int gx_grad_graphs(gx_handle* h, gx_memspace space, const int32_t* pred_label, float* edge_mask);
 
 /* ---- graph-classification mode (Explainer(..., graph_mode=True), explain_graphs: explain.py:80-85,356-363) ----
  * Batch of padded graphs, replacing Explainer(adj (G,n,n), feat (G,n,d), label (G)): block CSR over
