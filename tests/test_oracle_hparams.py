@@ -14,6 +14,7 @@ import torch
 
 import gnnx_oracle as O
 import kernel_spec as KS
+import mask_grad_oracle as MG
 import util
 import wide_oracle as WO
 from test_oracle_graph_variants import dense_m0, model_of
@@ -104,29 +105,8 @@ def test_cases_differ_from_the_defaults():
 # ------------------------------------------------------------------------------------ the specification under HSETS
 def _autograd_grads(A, X, gt, pl, idx, w, M, F, hp, graph_mode, bn):
     """torch autograd's dL/dM and dL/dF of the reference's loss (explain.py:665-808) at (M, F), float64."""
-    t = lambda a: torch.tensor(np.asarray(a), dtype=torch.float64)
-    L = 1
-    while ("W%d" % L) in w:
-        L += 1
-    W = dict(conv_w=[t(w["W%d" % l]) for l in range(1, L)], conv_b=[t(w["b%d" % l]) for l in range(1, L)], pred_w=t(w["Wp"]), pred_b=t(w["bp"]))
-    n = A.shape[0]
-    adj = t(A[None])
-    mask = t(M).requires_grad_(True)
-    fmask = t(F).requires_grad_(True)
-    S = torch.sigmoid(mask)
-    masked = adj * (S + S.t()) / 2 * (1 - torch.eye(n, dtype=torch.float64))
-    fm = torch.sigmoid(fmask)
-    ypred = O._gcn_forward_torch(t(X[None]) * fm, masked, W, graph_mode, bn)
-    res = torch.softmax(ypred[0] if graph_mode else ypred[-1, idx, :], dim=0)
-    m = torch.sigmoid(mask)
-    ent = -m * torch.log(m) - (1 - m) * torch.log(1 - m)
-    loss = -torch.log(res[int(gt)]) + hp.size * torch.sum(m) + hp.ent * torch.mean(ent) + hp.feat_size * torch.mean(fm)
-    if not graph_mode:
-        y = t(pl)
-        D = torch.diag(torch.sum(masked[0], 0))
-        loss = loss + hp.lap * (y @ (D - masked[0]) @ y) / adj.numel()
-    loss.backward()
-    return mask.grad.numpy(), fmask.grad.numpy()
+    g = MG.mask_grads(A, X, gt, pl, idx, w, M, F, hp, graph_mode=graph_mode, bn=bn)
+    return g.gM, g.gF
 
 
 def _node_problem(L, bn, node, seed):
