@@ -6,13 +6,27 @@ constrained path in oracle/gnnx_oracle.py (whose helpers they reuse):
   * explain_dense_torch  -- line-by-line port (dense tensors, torch autograd, torch.optim), bit-exact to the unmodified reference
                             (tests/golden/unconstrained_golden.npz, tools/gen_unconstrained_golden.py); the CPU baseline.
   * explain_closed_form  -- hand-derived forward / backward in numpy (fp64 or fp32): the specification csrc/explain_dense.cu implements.
-Both return the (n, n) float64 array the reference returns, masked_adj[0] * sub_adj (explain.py:209-211).
+Both return the (n, n) float64 array the reference returns, masked_adj[0] * sub_adj (explain.py:209-211), or with full=True the whole
+masked_adj[0] ExplainModule.forward built (the kernel's mask_dense output).
 """
 import math
 
 import numpy as np
 
 import gnnx_oracle as O
+
+
+def entry_classes(A):
+    """The off-diagonal entries of an (n, n) dense mask by class, {name: (rows, cols)}: "edge" the sub-adjacency slots, "nonedge" the
+    other pairs of rows that have an edge, "pad" the pairs with a row that has none (graph mode's padding and isolated rows).  Empty
+    classes are left out."""
+    A = np.asarray(A)
+    n = len(A)
+    live = (A != 0).any(1)
+    off = ~np.eye(n, dtype=bool)
+    both = live[:, None] & live[None, :]
+    cls = {"edge": off & (A != 0), "nonedge": off & (A == 0) & both, "pad": off & ~both}
+    return {k: np.nonzero(v) for k, v in cls.items() if v.any()}
 
 
 def _optimizer(hp, params):
@@ -37,11 +51,11 @@ def _optimizer(hp, params):
 
 
 def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0, hp=None, graph_mode=False, trace=None,
-                        bn=False):
+                        bn=False, full=False):
     """Port of Explainer.explain(..., unconstrained=True) (explain.py:97-146,209-211) with ExplainModule.{forward (unconstrained
     branch), loss, mask_density} (explain.py:680-808) inlined.  Arguments as gnnx_oracle.explain_dense_torch; M0 (n,n) float32, every
     entry of which is a parameter here.  trace: list receiving per epoch what print_training prints (loss, density, pred) and the terms.
-    mask_density keeps the CONSTRAINED _masked_adj (explain.py:680-683)."""
+    mask_density keeps the CONSTRAINED _masked_adj (explain.py:680-683).  full=True returns masked_adj[0] itself, all n^2 entries."""
     import torch
     hp = hp or O.default_hparams()
     W = weights if isinstance(weights, dict) and "conv_w" in weights else O.weights_to_torch(weights)
@@ -97,6 +111,8 @@ def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
             v = lambda t: float(t.detach()) if torch.is_tensor(t) else float(t)
             trace.append(dict(loss=v(loss), density=v(density), pred=res.detach().numpy().copy(), pred_loss=v(pred_loss),
                               lap=v(lap_loss), feat_size=v(feat_size_loss), size=v(size_loss), ent=v(mask_ent_loss)))
+    if full:
+        return masked_adj[0].detach().numpy().astype(np.float64)
     return masked_adj[0].detach().numpy() * np.asarray(sub_adj, dtype=np.float64)   # explain.py:209-211
 
 
@@ -132,11 +148,15 @@ def _opt_update(hp, t, f, P, G, m_, v_):
 
 
 def explain_closed_form(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0, hp=None, graph_mode=False, dtype=np.float64,
-                        return_state=False, bn=False):
-    """Hand-derived forward / backward of the unconstrained optimisation, any number of layers, --bn, every optimiser and scheduler.
+                        return_state=False, bn=False, full=False, trace=None):
+    """Hand-derived forward / backward of the unconstrained optimisation, any number of layers, --bn, an MLP prediction head
+    (weights["head"] = [(W, b), ..], torch's (out, in) layout, models.py:193-207), every optimiser and scheduler.
     The forward's adjacency is a = (1 - I) (.) (S + S^T)/2 with S = sigmoid(M) over all n^2 entries, the features are unmasked (so F is
     moved by feat_size alone), the Laplacian term covers every pair (node mode).  return_state=True also returns M, F and the
-    one-step gradients gM, gF of the last update (with num_epochs=1: the gradients at M0, F = 0)."""
+    one-step gradients gM, gF of the last update (with num_epochs=1: the gradients at M0, F = 0).  full=True returns the whole a
+    instead of a (.) sub_adj.  trace: list receiving per epoch dict(a=the epoch's dense mask, size=sum sigmoid(M), ent=sum H(sigmoid(M))
+    over all n^2 entries, feat=sum sigmoid(F)), the sums of the loss terms the kernel's trace reports (before that epoch's update), and
+    gM, the gradient of that epoch's update (absent from the last epoch unless return_state)."""
     hp = hp or O.default_hparams()
     f = dtype
     X = np.asarray(sub_feat, dtype=f)
@@ -154,6 +174,7 @@ def explain_closed_form(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
     offs = np.concatenate([[0], np.cumsum(dims)])
     Wp = np.asarray(weights["Wp"], dtype=f)
     bp = np.asarray(weights["bp"], dtype=f)
+    head = [(np.asarray(w, dtype=f), np.asarray(b, dtype=f)) for w, b in weights.get("head", [])]
     r = int(node_idx_new)
     M = np.asarray(M0, dtype=f).copy()
     mM = np.zeros_like(M); vM = np.zeros_like(M)
@@ -167,9 +188,11 @@ def explain_closed_form(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
     for t in range(1, hp.num_epochs + 1):
         S = O._sigmoid(M)
         a = A * (S + S.T) / 2                                                       # explain.py:688-692
+        sF = O._sigmoid(F)
+        if trace is not None:
+            trace.append(dict(a=a, size=float(S.sum()), ent=float((-S * np.log(S) - (1 - S) * np.log(1 - S)).sum()), feat=float(sF.sum())))
         if t == hp.num_epochs and not return_state:
             break
-        sF = O._sigmoid(F)
         H = [X]
         Yh, q, bn_state = [], [], []
         for l in range(L):
@@ -194,10 +217,15 @@ def explain_closed_form(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
             emb = np.concatenate(pooled)
         else:
             emb = np.concatenate([H[l + 1][r] for l in range(L)])
-        logits = Wp @ emb + bp
+        hs = [emb]
+        for w, b in head:                                                           # models.py:193-207: Linear, ReLU, .., Linear
+            hs.append(np.maximum(w @ hs[-1] + b, 0))
+        logits = Wp @ hs[-1] + bp
         p = np.exp(logits - logits.max()); p = p / p.sum()
         g = p.copy(); g[int(gt_label)] -= 1                                          # d(-log p[gt])/dlogits
         dEmb = Wp.T @ g
+        for k in range(len(head) - 1, -1, -1):
+            dEmb = head[k][0].T @ (dEmb * (hs[k + 1] > 0))
         for l in range(L):
             sl = dEmb[offs[l]:offs[l + 1]]
             if graph_mode:
@@ -220,9 +248,11 @@ def explain_closed_form(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
         gF = sF * (1 - sF) * (f(hp.feat_size) / f(d))                                # the forward never sees F
         # size = c*sum(S), ent = mean(H(S)) over ALL n^2 entries; the diagonal gets the regularisers only (A_ii = 0)
         gM = S * (1 - S) * ((A * dA + (A * dA).T) / 2 + f(hp.size) - f(hp.ent) * M / f(n * n))
+        if trace is not None:
+            trace[-1]["gM"] = gM
         for P, G, m_, v_ in ((M, gM, mM, vM), (F, gF, mF, vF)):
             _opt_update(hp, t, f, P, G, m_, v_)
-    out = a.astype(np.float64) * np.asarray(sub_adj, dtype=np.float64)
+    out = a.astype(np.float64) if full else a.astype(np.float64) * np.asarray(sub_adj, dtype=np.float64)
     if return_state:
         return out, dict(M=M, F=F, gM=gM, gF=gF)
     return out

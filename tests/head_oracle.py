@@ -85,11 +85,11 @@ def model_pred(adj, feat, weights, bn=False, graph_mode=False):
 
 
 def explain_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0, hp=None, graph_mode=False, bn=False,
-                  dtype=torch.float, unconstrained=False, return_feat=False):
+                  dtype=torch.float, unconstrained=False, return_feat=False, full=False):
     """Port of Explainer.explain's optimisation (explain.py:97-146,209-211; ExplainModule.forward :688-714, loss :740-808) in `dtype`.
     Arguments as gnnx_oracle.explain_dense_torch.  unconstrained: the dense mask sym(sigmoid(M)) (.) (1 - I) drives the forward and the
     features are not masked (explain.py:688-692).  Returns the (n, n) float64 masked adjacency times sub_adj (and, with return_feat,
-    sigmoid(feat_mask) as the last epoch's forward used it)."""
+    sigmoid(feat_mask) as the last epoch's forward used it).  full=True returns the whole masked adjacency, not times sub_adj."""
     hp = hp or O.default_hparams()
     W = to_torch(weights, dtype)
     n = sub_adj.shape[0]
@@ -132,5 +132,7 @@ def explain_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights
         opt.step()
         if sched is not None:
             sched.step()
-    out = masked[0].detach().numpy().astype(np.float64) * np.asarray(sub_adj, np.float64)
+    out = masked[0].detach().numpy().astype(np.float64)
+    if not full:
+        out = out * np.asarray(sub_adj, np.float64)
     return (out, fm_used.numpy().astype(np.float64)) if return_feat else out
