@@ -23,6 +23,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from .explain import _m0_at_edges, torch_m0_walk
+
 
 def shard_indices(num_items, world, rank, costs=None):
     """Positions (into the caller's node list) owned by `rank`.  With costs: sort by cost
@@ -128,7 +130,11 @@ def explain_nodes_sharded(explainer, node_indices, costs=None, group=None, use_e
         plan = eng.plan_nodes(nodes[pos], explainer.n_hops, fetch=(init == "torch"))
         m0_dev = None
         if init == "torch":   # every rank walks the whole list so that torch's RNG is consumed exactly as one process would
-            m0_dev = torch.from_numpy(explainer._draw_m0_subset(plan, n_all, pos)).to(dev)
+            mine = set(pos.tolist())
+            walk = enumerate(torch_m0_walk(n_all))
+            m0_dev = torch.from_numpy(_m0_at_edges(plan, (M for p, M in walk if p in mine))).to(dev)
+            for _ in walk:
+                pass
         local = eng.explain_nodes_device(hp, m0_dev)
     else:
         plan, local = None, torch.zeros(0, dtype=torch.float32, device=dev)

@@ -86,6 +86,29 @@ def model_weights(model):
     return w, len(names)
 
 
+def torch_m0_walk(sizes):
+    """The torch-compatible initial masks (args.gnnx_init="torch") of a list, drawn lazily in list order: per size n the float32 (n, n)
+    array FloatTensor(n, n).normal_(1, std) of ExplainModule.construct_edge_mask (explain.py:645-652), a view of the drawn tensor.  n is
+    the k-hop size in node mode and the padded max_nodes in graph mode.  The reference draws for every entry it explains, so every entry
+    is drawn here too, used or not (another rank's entries, the gradient baseline): once the walk is exhausted torch's global CPU RNG is
+    where the reference's loop over the same list leaves it.  The n^2 normals per entry are this policy's cost (~3 ns each on one core;
+    args.gnnx_init="device" has no host work)."""
+    for n in sizes:
+        n = int(n)
+        yield torch.FloatTensor(n, n).normal_(1.0, torch.nn.init.calculate_gain("relu") * math.sqrt(2.0 / (n + n))).numpy()
+
+
+def _m0_at_edges(plan, draws):
+    """M0 of a node plan at its directed-edge slots (float32[total_edges]): the next plan.count arrays of the iterator `draws`, one per
+    task in plan order, each gathered at its task's slots."""
+    m0 = np.empty(plan.total_edges, dtype=np.float32)
+    flat = plan.flat_index()            # row * n + col of every edge slot, whole batch at once
+    eo = plan.edge_off
+    for t in range(plan.count):
+        np.take(next(draws).reshape(-1), flat[eo[t]:eo[t + 1]], out=m0[eo[t]:eo[t + 1]])
+    return m0
+
+
 class Explainer:
     def __init__(self, model, adj, feat, label, pred, train_idx, args, writer=None,
                  print_training=True, graph_mode=False, graph_idx=False, device=None):
@@ -125,16 +148,13 @@ class Explainer:
                               head=weights.get("head"))
         if getattr(args, "gnnx_latency", False):
             self.engine.debug_cluster(0, 0)   # latency mode: thread-block clusters for the expensive tasks of batches that leave SMs idle
-        # model / optimiser variants run in the variant kernel, which does not log the per-epoch trace print_training replays: the
-        # selection of gx_set_model (--bn, num_gc_layers != 3, hidden or output widths above 32, inputs wider than 128, attention)
-        # and every optimiser other than Adam
         self._max_width = max(weights["W%d" % l].shape[1] for l in range(1, num_layers + 1))
         self._wide_layers = self._max_width > 32
-        self._no_trace = (bn or num_layers != 3 or self._wide_layers or getattr(args, "opt", "adam") != "adam" or self._att
-                          or self._wide or self._head)
-        # the models the tuned kernels run (the gradient baseline's coverage): 3 layers, widths <= 32, no --bn / attention / head,
-        # inputs up to 128 features
+        # the models the tuned kernels do not run (outside the gradient baseline's coverage), gx_set_model's selection of the variant
+        # kernel: --bn, num_gc_layers != 3, hidden or output widths above 32, attention, inputs wider than 128, an MLP head
         self._variant = bn or num_layers != 3 or self._wide_layers or self._att or self._wide or self._head
+        # the variant kernel does not log the per-epoch trace print_training replays, nor does any optimiser other than Adam
+        self._no_trace = self._variant or getattr(args, "opt", "adam") != "adam"
         # node mode also takes a scipy.sparse (N,N) adjacency, a batch of one graph (feat / label / pred keep their (1,N,..) shapes): a
         # graph of 10^5 nodes has 10^10 dense entries, its CSR comes straight from the sparse matrix
         self._sparse = _gu.is_sparse(adj)
@@ -235,56 +255,15 @@ class Explainer:
             hp.opt_restart = int(a.opt_restart)
         return hp, init
 
-    def _draw_m0(self, plan, keep_dense=False):
-        """Per node, in call order: FloatTensor(n,n).normal_(1, std) (explain.py:645-652), gathered at the
-        directed-edge slots.  Consumes torch's global CPU RNG exactly like the reference (the n^2 draw per node IS the
-        cost of this policy: ~3 ns per normal on one core; args.gnnx_init="device" has no host work).
-        keep_dense: also return the dense draws (the off-edge entries only matter for the printed loss)."""
-        m0 = np.empty(plan.total_edges, dtype=np.float32)
-        gain = torch.nn.init.calculate_gain("relu")
-        flat = plan.flat_index()            # row * n + col of every edge slot, whole batch at once
-        dense = [] if keep_dense else None
-        for t in range(plan.count):
-            n = plan.n(t)
-            std = gain * math.sqrt(2.0 / (n + n))
-            M = torch.FloatTensor(n, n).normal_(1.0, std).numpy()
-            np.take(M.reshape(-1), flat[plan.edge_off[t]:plan.edge_off[t + 1]], out=m0[plan.edge_off[t]:plan.edge_off[t + 1]])
-            if keep_dense:
-                dense.append(M)
-        return (m0, dense) if keep_dense else m0
-
-    def _draw_m0_subset(self, plan, n_all, positions):
-        """Sharded runs with the torch-compatible init: walk the WHOLE node list in order (n_all[p] = sub-graph size of list entry
-        p, from gx_count_nodes) drawing every node's n^2 normals like one process would, and keep the edge entries of the entries
-        this rank owns (`positions`, ascending; `plan` is the plan of exactly those nodes)."""
-        m0 = np.empty(plan.total_edges, dtype=np.float32)
-        gain = torch.nn.init.calculate_gain("relu")
-        flat = plan.flat_index()
-        mine = {int(p): t for t, p in enumerate(positions)}
-        for p, n in enumerate(n_all):
-            n = int(n)
-            M = torch.FloatTensor(n, n).normal_(1.0, gain * math.sqrt(2.0 / (n + n)))
-            t = mine.get(p)
-            if t is not None:
-                np.take(M.numpy().reshape(-1), flat[plan.edge_off[t]:plan.edge_off[t + 1]], out=m0[plan.edge_off[t]:plan.edge_off[t + 1]])
-        return m0
-
     @staticmethod
     def _draw_graph_m0_subset(n, num_graphs, positions, rows_cols):
-        """Graph mode's counterpart for sharded runs: walk the WHOLE graph list (num_graphs entries) drawing FloatTensor(n, n).normal_(1,
-        std) per graph, n = the padded size, exactly as _explain_graph_batch does, and keep M[rows, cols] of the entries this rank owns
-        (`positions`, ascending; rows_cols[i] = (rows, cols) of positions[i]'s graph in slot order), concatenated -> float32.  torch's
-        global RNG ends where one process's explain_graphs of the same list leaves it, whatever the rank owns."""
-        std = torch.nn.init.calculate_gain("relu") * math.sqrt(2.0 / (n + n))
-        mine = {int(p): i for i, p in enumerate(positions)}
-        parts = [None] * len(mine)
-        for p in range(int(num_graphs)):
-            M = torch.FloatTensor(n, n).normal_(1.0, std)
-            i = mine.get(p)
-            if i is not None:
-                rows, cols = rows_cols[i]
-                parts[i] = M.numpy()[rows, cols]
-        return np.concatenate(parts).astype(np.float32, copy=False) if parts else np.zeros(0, np.float32)
+        """Graph mode's M0 on one rank of a sharded run: the walk over the WHOLE graph list (num_graphs graphs padded to n), keeping
+        M[rows, cols] of the graphs at `positions` (ascending; rows_cols[i] = (rows, cols) of positions[i]'s graph in slot order),
+        concatenated -> float32.  torch's global RNG ends where one process's explain_graphs of the same list leaves it, whatever the
+        rank owns."""
+        kept = dict(zip((int(p) for p in positions), rows_cols))
+        parts = [M[kept[p]] for p, M in enumerate(torch_m0_walk([n] * int(num_graphs))) if p in kept]
+        return np.concatenate(parts) if parts else np.zeros(0, np.float32)
 
     def _explain_batch(self, node_indices, graph_idx=0, model="exp", unconstrained=False):
         if model not in ("exp", "grad"):
@@ -293,6 +272,7 @@ class Explainer:
         nodes = [int(i) for i in node_indices]
         plan = self.engine.plan_nodes(nodes, self.n_hops)
         edge_mask = np.empty(plan.total_edges, dtype=np.float32)
+        draws = torch_m0_walk(np.diff(plan.node_off))     # lazy: draws nothing unless the torch init reads it below
         if model == "grad":        # explain.py:125-133: one backward to the adjacency, no mask parameters
             if self._head:
                 raise NotImplementedError("model='grad' is not built for models with an MLP prediction head (pred_hidden_dims)")
@@ -303,17 +283,14 @@ class Explainer:
                     raise NotImplementedError(str(e)) from None
                 raise
             if self._hparams()[1] == "torch":      # the reference still constructs an ExplainModule per node, i.e. consumes n^2 normals:
-                self._draw_m0(plan)                # keep the RNG in step
+                for _ in draws:                    # keep the RNG in step
+                    pass
             return plan, edge_mask
-        if unconstrained and self._att:
-            raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
-        if unconstrained and self._wide:
-            raise NotImplementedError("unconstrained=True is not built for inputs wider than 128 features")
-        self._check_unconstrained_width(unconstrained)
+        self._check_unconstrained(unconstrained)
         hp, init = self._hparams()
         if unconstrained:
             # explain.py:688-692: the dense mask drives the forward, so every one of the n^2 normals of M0 is a parameter
-            m0 = np.concatenate([D.reshape(-1) for D in self._draw_m0(plan, keep_dense=True)[1]]) if init == "torch" else None
+            m0 = np.concatenate([D.reshape(-1) for D in draws]) if init == "torch" else None
             if not self.print_training:
                 self.engine.explain_nodes_unconstrained(hp, m0, edge_mask)
                 return plan, edge_mask
@@ -325,11 +302,13 @@ class Explainer:
         if not self.print_training or self._no_trace:
             if self.print_training:
                 self._print_no_trace()
-            m0 = self._draw_m0(plan) if init == "torch" else None
+            m0 = _m0_at_edges(plan, draws) if init == "torch" else None
             self.engine.explain_nodes_host(hp, m0, edge_mask)
             return plan, edge_mask
-        # print_training (explain.py:148-159): the kernels log every epoch's loss terms / density / softmax row (gx_explain_io.trace)
-        m0, dense = self._draw_m0(plan, keep_dense=True) if init == "torch" else (None, None)
+        # print_training (explain.py:148-159): the kernels log every epoch's loss terms / density / softmax row (gx_explain_io.trace); the
+        # off-edge entries of the dense draws only matter for the printed loss
+        dense = list(draws) if init == "torch" else None
+        m0 = None if dense is None else _m0_at_edges(plan, iter(dense))
         trace = np.zeros((plan.count, hp.num_epochs, _abi.GX_TRACE_COLS), np.float32)
         pred = np.zeros((plan.count, hp.num_epochs, self.engine.num_classes), np.float32)
         self.engine.explain_nodes_ex(hp, m0, edge_mask, trace=trace, trace_pred=pred)
@@ -337,8 +316,14 @@ class Explainer:
         self.last_trace = self._print_trace(hp, trace, pred, off, np.diff(plan.node_off).astype(np.float64) ** 2)
         return plan, edge_mask
 
-    def _check_unconstrained_width(self, unconstrained):
-        if unconstrained and self._max_width > 128:
+    def _check_unconstrained(self, unconstrained):
+        if not unconstrained:
+            return
+        if self._att:
+            raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
+        if self._wide:
+            raise NotImplementedError("unconstrained=True is not built for inputs wider than 128 features")
+        if self._max_width > 128:
             raise NotImplementedError("unconstrained=True is not built for hidden / output widths above 128 (this model: %d)" % self._max_width)
 
     def _print_no_trace(self):
@@ -380,11 +365,7 @@ class Explainer:
     _MAX_TRACE_EPOCHS = 1536
 
     def _explain_graph_batch(self, graph_indices, unconstrained=False):
-        if unconstrained and self._att:
-            raise NotImplementedError("unconstrained=True is not built for attention models (--method att)")
-        if unconstrained and self._wide:
-            raise NotImplementedError("unconstrained=True is not built for inputs wider than 128 features")
-        self._check_unconstrained_width(unconstrained)
+        self._check_unconstrained(unconstrained)
         gids = [int(g) for g in graph_indices]
         edge_off = self.engine.plan_graphs(gids)
         hp, init = self._hparams()
@@ -401,19 +382,11 @@ class Explainer:
         dense = None      # the full (n, n) draws: the unconstrained kernel's M0, or the off-edge entries of the printed loss
         rc = [self.engine.graph_rows_cols(g) for g in gids]
         if init == "torch":
+            draws = torch_m0_walk([n] * len(gids))      # n = the padded size
             if unconstrained or traced:
-                dense = np.empty(n * n * len(gids), dtype=np.float32)
-            if not unconstrained:
-                m0 = np.empty(int(edge_off[-1]), dtype=np.float32)
-            std = torch.nn.init.calculate_gain("relu") * math.sqrt(2.0 / (n + n))
-            for t, (rows, cols) in enumerate(rc):
-                M = torch.FloatTensor(n, n).normal_(1.0, std).numpy()      # explain.py:645-652, n = padded size
-                if dense is not None:
-                    dense[t * n * n:(t + 1) * n * n] = M.reshape(-1)
-                if m0 is not None:
-                    m0[edge_off[t]:edge_off[t + 1]] = M[rows, cols]
-            if unconstrained:
-                m0 = dense
+                dense = np.concatenate([M.reshape(-1) for M in draws])
+                draws = dense.reshape(-1, n, n)
+            m0 = dense if unconstrained else np.concatenate([M[rows_cols] for M, rows_cols in zip(draws, rc)])
         edge_mask = np.empty(int(edge_off[-1]), dtype=np.float32)
         trace = pred = None
         if traced:
@@ -463,7 +436,8 @@ class Explainer:
         labels = self._graph_grad_labels(gids)
         if self._hparams()[1] == "torch":
             # the reference still constructs an ExplainModule per graph, i.e. draws its n^2 normals (explain.py:645-652): keep the RNG in step
-            self._draw_graph_m0_subset(self.engine.batch_n, len(gids), [], [])
+            for _ in torch_m0_walk([self.engine.batch_n] * len(gids)):
+                pass
         edge_mask = np.empty(max(int(edge_off[-1]), 1), dtype=np.float32)
         try:
             self.engine.grad_graphs_host(labels, edge_mask)
@@ -529,7 +503,7 @@ class Explainer:
             dev = torch.device("cuda", eng.device)
             m0_dev = None
             if init == "torch":
-                m0_dev = torch.from_numpy(self._draw_m0(plan)).to(dev, non_blocking=False)
+                m0_dev = torch.from_numpy(_m0_at_edges(plan, torch_m0_walk(np.diff(plan.node_off)))).to(dev, non_blocking=False)
             mask_dev = eng.explain_nodes_device(hp, m0_dev)
             dense_dev = eng.densify_device(mask_dev)
             if copy:
@@ -684,7 +658,6 @@ class Explainer:
         if int(threshold_num) < 1:
             raise ValueError("threshold_num must be >= 1")
         hp, init = self._hparams()
-        gain = torch.nn.init.calculate_gain("relu")
         clock = [time.perf_counter()]
 
         def tick(key):
@@ -695,7 +668,10 @@ class Explainer:
                 clock[0] = now
 
         thr_p, cnt_p, uv_p, val_p = [], [], [], []
-        walk = 0          # first list entry whose normals have not been drawn
+        if init == "torch":
+            # the walk reads an entry's size when it reaches the entry: a chunk's own plan fills in the sizes of its positions first
+            sizes = np.zeros(len(nodes), np.int64) if n_all is None else np.array(n_all, np.int64)
+            walk = enumerate(torch_m0_walk(sizes[p] for p in range(len(nodes))))
         latency = bool(getattr(self.args, "gnnx_latency", False))
         if latency:
             eng.debug_cluster(1, 0)
@@ -707,18 +683,9 @@ class Explainer:
                 tick("plan")
                 m0_dev = None
                 if init == "torch":
-                    m0 = np.empty(plan.total_edges, dtype=np.float32)
-                    flat = plan.flat_index()
-                    eo = plan.edge_off
-                    mine = {int(p): t for t, p in enumerate(pos)}
-                    for p in range(walk, int(pos[-1]) + 1):
-                        t = mine.get(p)
-                        n = plan.n(t) if t is not None else int(n_all[p])
-                        M = torch.FloatTensor(n, n).normal_(1.0, gain * math.sqrt(2.0 / (n + n)))
-                        if t is not None:
-                            np.take(M.numpy().reshape(-1), flat[eo[t]:eo[t + 1]], out=m0[eo[t]:eo[t + 1]])
-                    walk = int(pos[-1]) + 1
-                    m0_dev = torch.from_numpy(m0).to(dev)
+                    sizes[pos] = np.diff(plan.node_off)
+                    mine = set(pos.tolist())
+                    m0_dev = torch.from_numpy(_m0_at_edges(plan, (M for p, M in walk if p in mine))).to(dev)
                     tick("m0")
                 mask = eng.explain_nodes_device(hp, m0_dev)
                 if timings is not None:
@@ -735,9 +702,8 @@ class Explainer:
             if latency:
                 eng.debug_cluster(0, 0)
         if init == "torch":      # the rest of the list, so that torch's RNG ends as after one process's explain_nodes
-            for p in range(walk, len(nodes)):
-                n = int(n_all[p])
-                torch.FloatTensor(n, n).normal_(1.0, gain * math.sqrt(2.0 / (n + n)))
+            for _ in walk:
+                pass
         if not thr_p:
             return (torch.zeros(0, dtype=torch.float32, device=dev), np.zeros(0, np.int64),
                     torch.zeros((0, 2), dtype=torch.int32, device=dev), torch.zeros(0, dtype=torch.float32, device=dev))

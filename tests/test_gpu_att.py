@@ -229,7 +229,7 @@ def test_explainer_dropin_node_mode(tmp_path, capsys, L, bn):
     for node, got in zip(nodes, many):
         A, X, gt, pl, idx = _sub(s, node)
         n = A.shape[0]
-        M0 = torch.FloatTensor(n, n).normal_(1.0, torch.nn.init.calculate_gain("relu") * np.sqrt(2.0 / (n + n))).numpy()
+        M0 = O.draw_m0(n)
         port = AO.explain_att_torch(A, X, s.label[node], pl, idx, s.w, M0, O.default_hparams(num_epochs=20), bn=bn)
         p64 = AO.explain_att_torch(A, X, s.label[node], pl, idx, s.w, M0, O.default_hparams(num_epochs=20), bn=bn, dtype=torch.float64)
         assert O.rel_l2(got, port) <= max(1e-4, 3 * O.rel_l2(p64, port)), node
@@ -259,9 +259,8 @@ def test_explainer_dropin_graph_mode(tmp_path, capsys):
     torch.manual_seed(4)
     got = ex.explain_graphs(gids)
     torch.manual_seed(4)
-    std = torch.nn.init.calculate_gain("relu") * np.sqrt(2.0 / (n + n))
     for g, masked in zip(gids, got):
-        M0 = torch.FloatTensor(n, n).normal_(1.0, std).numpy()
+        M0 = O.draw_m0(n)
         A = np.asarray(gg["adj"][g], np.float64)
         port = AO.explain_att_torch(A, gg["feat"][g], label[g], None, 0, w, M0, O.default_hparams(num_epochs=20), graph_mode=True)
         p64 = AO.explain_att_torch(A, gg["feat"][g], label[g], None, 0, w, M0, O.default_hparams(num_epochs=20), graph_mode=True,

@@ -383,7 +383,7 @@ def test_explainer_dropin_node_mode(tmp_path, capsys, hid, emb):
     for node, got in zip(nodes, many):
         A, X, gt, pl, idx = _sub(s, node)
         n = A.shape[0]
-        M0 = torch.FloatTensor(n, n).normal_(1.0, torch.nn.init.calculate_gain("relu") * np.sqrt(2.0 / (n + n))).numpy()
+        M0 = O.draw_m0(n)
         hp = O.default_hparams(num_epochs=20)
         port = WO.explain_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True)
         p64 = WO.explain_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True, dtype=torch.float64)
@@ -409,9 +409,8 @@ def test_explainer_dropin_graph_mode(tmp_path, capsys):
     torch.manual_seed(4)
     got = ex.explain_graphs(gids)
     torch.manual_seed(4)
-    std = torch.nn.init.calculate_gain("relu") * np.sqrt(2.0 / (n + n))
     for g, masked in zip(gids, got):
-        M0 = torch.FloatTensor(n, n).normal_(1.0, std).numpy()
+        M0 = O.draw_m0(n)
         A = np.asarray(adj[g], np.float64)
         hp = O.default_hparams(num_epochs=20)
         port = WO.explain_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True)

@@ -251,9 +251,8 @@ def _explainer(gg, args, pred, bn=False, L=3):
 
 def _normals_after(seed, n, count):
     torch.manual_seed(seed)
-    std = torch.nn.init.calculate_gain("relu") * np.sqrt(2.0 / (n + n))
     for _ in range(count):
-        torch.FloatTensor(n, n).normal_(1.0, std)
+        O.draw_m0(n)
     return torch.get_rng_state()
 
 
