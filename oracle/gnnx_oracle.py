@@ -11,9 +11,10 @@ UNMODIFIED reference in the authoring container, and tests/test_oracle.py checks
 below against them.
 
 Two restatements of the mask optimisation are kept on purpose:
-  * explain_dense_torch  -- line-by-line port (dense n x n tensors, torch autograd, torch.optim.Adam),
-                            i.e. the reference's own cost structure; this is the CPU baseline
-                            ("port") that bench.py times.
+  * explain_dense_torch  -- line-by-line port (dense n x n tensors, torch autograd, torch.optim), i.e. the reference's own
+                            cost structure, for every model variant (--bn, any number of layers, attention, MLP heads),
+                            unconstrained=True and any dtype; this is the CPU baseline ("port") that bench.py times, and
+                            the one port every test compares against.
   * explain_closed_form  -- hand-derived forward/backward in numpy (fp64 or fp32) with parameters
                             that matter only on the directed edges; this is the specification the
                             CUDA kernel implements (SURVEY.md section 8a "validated edge-list spec").
@@ -207,17 +208,23 @@ def set_pool(fn):
 
 def _gcn_forward_torch(x, adj, W, graph_mode, bn=False):
     """models.py:58-80 (GraphConv.forward), :230-267 (gcn_forward), :363-376 (node readout),
-    :269-316 (graph readout).  x (1,n,d), adj (1,n,n).  Any number of layers (len(W["conv_w"]) =
+    :269-316 (graph readout), :193-207 (pred_model).  x (1,n,d), adj (1,n,n).  Any number of layers (len(W["conv_w"]) =
     args.num_gc_layers).  bn=True: models.py:222-228,242-243,252-253 -- a FRESH BatchNorm1d(n) in train mode
     after the ReLU of every layer but the last, i.e. each node's row is standardised over its features
-    (biased variance, eps 1e-5, no affine)."""
+    (biased variance, eps 1e-5, no affine).  W["att_w"] (--method att): every layer scales the adjacency it is given by the
+    unnormalised scores P P^T, P = H_{l-1} Wa_l (models.py:62-68).  W["head"] (pred_hidden_dims): Linear, ReLU, .. before the last
+    Linear (W["pred_w"], W["pred_b"])."""
     import torch
     import torch.nn.functional as F
     outs = []
     h = x
     L = len(W["conv_w"])
     for l in range(L):
-        y = torch.matmul(adj, h)                       # models.py:70
+        a = adj
+        if W.get("att_w") is not None:
+            x_att = torch.matmul(h, W["att_w"][l])     # models.py:63
+            a = adj * (x_att @ x_att.permute(0, 2, 1))  # models.py:66-68
+        y = torch.matmul(a, h)                         # models.py:70
         y = torch.matmul(y, W["conv_w"][l])            # models.py:71
         if W["conv_b"][l] is not None:
             y = y + W["conv_b"][l]                     # models.py:76
@@ -229,19 +236,32 @@ def _gcn_forward_torch(x, adj, W, graph_mode, bn=False):
         outs.append(y)
         h = y
     if graph_mode:
-        pooled = max_pool(outs)                                    # models.py:283,293,304
-        emb = torch.cat(pooled, dim=1)                             # models.py:309
-        return F.linear(emb, W["pred_w"], W["pred_b"])             # (1,C)
-    emb = torch.cat(outs, dim=2)                                   # models.py:260
-    return F.linear(emb, W["pred_w"], W["pred_b"])                 # (1,n,C) models.py:375
+        emb = torch.cat(max_pool(outs), dim=1)                     # models.py:283,293,304,309
+    else:
+        emb = torch.cat(outs, dim=2)                               # models.py:260
+    for w, b in W.get("head", ()):
+        emb = torch.relu(F.linear(emb, w, b))                      # models.py:193-207
+    return F.linear(emb, W["pred_w"], W["pred_b"])                 # (1,C) graph mode, (1,n,C) node mode (models.py:375)
 
 
-def weights_to_torch(weights, requires_grad=True):
-    """weights: dict with W1,b1,W2,b2,W3,b3,Wp,bp (numpy) -> the structure _gcn_forward_torch uses.
-    requires_grad=True mirrors the reference, whose frozen model is a registered sub-module of
+def head_layers(weights):
+    """The hidden head Linears [(W, b), ..]: weights["head"], or the fixture's Wh1 / bh1, Wh2 / bh2, .."""
+    if "head" in weights:
+        return list(weights["head"])
+    out, j = [], 1
+    while ("Wh%d" % j) in weights:
+        out.append((weights["Wh%d" % j], weights["bh%d" % j]))
+        j += 1
+    return out
+
+
+def weights_to_torch(weights, requires_grad=True, dtype=None):
+    """weights: dict with W1,b1,..,WL,bL,Wp,bp (numpy) -> the structure _gcn_forward_torch uses, in dtype (None: torch.float).
+    Wa1..WaL (attention) become "att_w"; the head's hidden Linears (head_layers, torch's (out, in) layout) become "head", and Wp / bp
+    are then the last Linear.  requires_grad=True mirrors the reference, whose frozen model is a registered sub-module of
     ExplainModule (explain.py:598) so autograd also computes the (unused) weight gradients."""
     import torch
-    t = lambda a: torch.tensor(np.asarray(a), dtype=torch.float, requires_grad=requires_grad)
+    t = lambda a: torch.tensor(np.asarray(a), dtype=dtype or torch.float, requires_grad=requires_grad)
     conv_w, conv_b = [], []
     l = 1
     while ("W%d" % l) in weights:
@@ -249,36 +269,34 @@ def weights_to_torch(weights, requires_grad=True):
         b = weights.get("b%d" % l)
         conv_b.append(None if b is None else t(b))
         l += 1
-    return dict(conv_w=conv_w, conv_b=conv_b, pred_w=t(weights["Wp"]), pred_b=t(weights["bp"]))
+    W = dict(conv_w=conv_w, conv_b=conv_b, pred_w=t(weights["Wp"]), pred_b=t(weights["bp"]))
+    if "Wa1" in weights:
+        W["att_w"] = [t(weights["Wa%d" % l]) for l in range(1, len(conv_w) + 1)]
+    head = head_layers(weights)
+    if head:
+        W["head"] = [(t(w), t(b)) for w, b in head]
+    return W
 
 
-def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0,
-                        hp=None, graph_mode=False, trace=None, bn=False, return_feat=False):
-    """Port of Explainer.explain's optimisation (explain.py:97-146,209-211) with
-    ExplainModule.{_masked_adj,forward,loss,mask_density} (explain.py:665-808) inlined.
-
-    sub_adj (n,n) 0/1; sub_feat (n,d); gt_label = label[0][node_idx] (node) or the graph label;
-    pred_label (n,) int = argmax(pred[nbrs]) (node mode; unused in graph mode); M0 (n,n) float32.
-    Returns the (n,n) float64 array the reference returns (masked_adj[0] * sub_adj); return_feat=True also
-    returns sigmoid(feat_mask) as the last epoch's forward used it (after num_epochs - 1 updates), float64 (d,)."""
+def model_pred(adj, feat, weights, bn=False, graph_mode=False):
+    """GcnEncoderNode / GcnEncoderGraph.forward on the raw adjacency (self loops included): the `pred` of the checkpoint, float32."""
     import torch
-    hp = hp or default_hparams()
-    W = weights if isinstance(weights, dict) and "conv_w" in weights else weights_to_torch(weights)
-    n = sub_adj.shape[0]
-    adj = torch.tensor(np.asarray(sub_adj)[None], dtype=torch.float)            # explain.py:97
-    x = torch.tensor(np.asarray(sub_feat)[None], requires_grad=True, dtype=torch.float)  # :98
-    mask = torch.nn.Parameter(torch.tensor(np.asarray(M0), dtype=torch.float))  # explain.py:646-652
-    feat_mask = torch.nn.Parameter(torch.zeros(x.size(-1)))                     # explain.py:633-643
-    diag_mask = torch.ones(n, n) - torch.eye(n)                                 # explain.py:617
-    # utils/train_utils.py:7-23 (build_optimizer; explain.py:622)
+    with torch.no_grad():
+        return _gcn_forward_torch(torch.tensor(np.asarray(feat, np.float32)[None]), torch.tensor(np.asarray(adj, np.float32)[None]),
+                                  weights_to_torch(weights, requires_grad=False), graph_mode, bn)[0].numpy()
+
+
+def build_optimizer(hp, params):
+    """utils/train_utils.py:7-23 (build_optimizer; explain.py:622) -> (optimizer, scheduler or None)."""
+    import torch
     if hp.opt == "adam":
-        opt = torch.optim.Adam([mask, feat_mask], lr=hp.lr, betas=(hp.beta1, hp.beta2), eps=hp.eps)
+        opt = torch.optim.Adam(params, lr=hp.lr, betas=(hp.beta1, hp.beta2), eps=hp.eps)
     elif hp.opt == "sgd":
-        opt = torch.optim.SGD([mask, feat_mask], lr=hp.lr, momentum=0.95)
+        opt = torch.optim.SGD(params, lr=hp.lr, momentum=0.95)
     elif hp.opt == "rmsprop":
-        opt = torch.optim.RMSprop([mask, feat_mask], lr=hp.lr)
+        opt = torch.optim.RMSprop(params, lr=hp.lr)
     elif hp.opt == "adagrad":
-        opt = torch.optim.Adagrad([mask, feat_mask], lr=hp.lr)
+        opt = torch.optim.Adagrad(params, lr=hp.lr)
     else:
         raise ValueError(hp.opt)
     sched = None
@@ -286,62 +304,111 @@ def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, w
         sched = torch.optim.lr_scheduler.StepLR(opt, step_size=hp.opt_decay_step, gamma=hp.opt_decay_rate)
     elif hp.opt_scheduler == "cos":
         sched = torch.optim.lr_scheduler.CosineAnnealingLR(opt, T_max=hp.opt_restart)
-    params = [mask, feat_mask] + W["conv_w"] + [b for b in W["conv_b"] if b is not None] + [W["pred_w"], W["pred_b"]]
-    pred_label_t = None if graph_mode else torch.tensor(np.asarray(pred_label), dtype=torch.float)
+    return opt, sched
 
-    def masked_adj_fn():                                                        # explain.py:665-678
-        sym = torch.sigmoid(mask)
-        sym = (sym + sym.t()) / 2
-        return adj * sym * diag_mask
 
-    masked_adj = None
-    for epoch in range(hp.num_epochs):                                          # explain.py:137
-        for p in params:
+def _sym(mask):
+    import torch
+    sym = torch.sigmoid(mask)                                                   # explain.py:671-676
+    return (sym + sym.t()) / 2
+
+
+def _epoch_loss(mask, feat_mask, adj, x, diag_mask, W, gt_label, pred_label_t, node_idx_new, hp, graph_mode=False, bn=False,
+                unconstrained=False):
+    """ExplainModule.{_masked_adj,forward,loss} (explain.py:665-808) at mask parameters `mask` (n,n) and `feat_mask` (d,):
+    adj (1,n,n), x (1,n,d), diag_mask (n,n), pred_label_t (n,) the Laplacian term's labels (node mode).
+    The operations run in the reference's order: autograd sums a tensor's gradient contributions in the order of their creation, so
+    the order is part of the bits.  In particular sigmoid(feat_mask) and sigmoid(mask) are evaluated afresh for the regularisers.
+    unconstrained=True: the forward's adjacency is the dense sym(sigmoid(M)) (.) (1 - I) and the features are not masked
+    (explain.py:688-692).  Returns (loss, masked_adj, res, terms) with res the softmax the prediction loss reads and terms the
+    loss terms plus m = sigmoid(mask), mask_ent (n,n) and fm = sigmoid(feat_mask)."""
+    import torch
+    sym = _sym(mask)
+    if unconstrained:
+        masked_adj = torch.unsqueeze(sym, 0) * diag_mask                        # explain.py:688-692
+        ypred = _gcn_forward_torch(x, masked_adj, W, graph_mode, bn)            # explain.py:709, raw features
+    else:
+        masked_adj = adj * sym * diag_mask                                      # explain.py:678,694
+        ypred = _gcn_forward_torch(x * torch.sigmoid(feat_mask), masked_adj, W, graph_mode, bn)   # explain.py:695-709
+    if graph_mode:
+        res = torch.softmax(ypred[0], dim=0)                                    # explain.py:711
+    else:
+        res = torch.softmax(ypred[-1, node_idx_new, :], dim=0)                  # explain.py:713-714
+    pred_loss = -torch.log(res[int(gt_label)])                                  # explain.py:750-753
+    m = torch.sigmoid(mask)                                                     # explain.py:756-757
+    size_loss = hp.size * torch.sum(m)                                          # explain.py:760
+    fm = torch.sigmoid(feat_mask)
+    feat_size_loss = hp.feat_size * torch.mean(fm)                              # explain.py:764-766
+    mask_ent = -m * torch.log(m) - (1 - m) * torch.log(1 - m)                   # explain.py:769
+    mask_ent_loss = hp.ent * torch.mean(mask_ent)                               # explain.py:770
+    if graph_mode:
+        lap_loss = 0                                                            # explain.py:787-788
+    else:
+        D = torch.diag(torch.sum(masked_adj[0], 0))                             # explain.py:780
+        Lm = D - masked_adj[-1]                                                 # explain.py:781-782
+        lap_loss = hp.lap * (pred_label_t @ Lm @ pred_label_t) / adj.numel()    # explain.py:789-793
+    loss = pred_loss + size_loss + lap_loss + mask_ent_loss + feat_size_loss    # explain.py:808
+    terms = dict(pred_loss=pred_loss, size=size_loss, feat_size=feat_size_loss, ent=mask_ent_loss, lap=lap_loss, m=m, mask_ent=mask_ent,
+                 fm=fm)
+    return loss, masked_adj, res, terms
+
+
+def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0, hp=None, graph_mode=False, trace=None,
+                        bn=False, return_feat=False, dtype=None, unconstrained=False, full=False):
+    """Port of Explainer.explain's optimisation (explain.py:97-146,209-211) with
+    ExplainModule.{_masked_adj,forward,loss,mask_density} (explain.py:665-808) inlined, in dtype (None: torch.float), for every model
+    _gcn_forward_torch runs (weights as weights_to_torch reads them, or already converted).
+
+    sub_adj (n,n) 0/1; sub_feat (n,d); gt_label = label[0][node_idx] (node) or the graph label;
+    pred_label (n,) int = argmax(pred[nbrs]) (node mode; unused in graph mode); M0 (n,n) float32.
+    unconstrained=True: Explainer.explain(..., unconstrained=True), every entry of M0 a parameter (_epoch_loss).
+    Returns the (n,n) float64 array the reference returns (masked_adj[0] * sub_adj), with full=True the whole masked_adj[0];
+    return_feat=True also returns sigmoid(feat_mask) as the last epoch's forward used it (after num_epochs - 1 updates), float64 (d,).
+    trace: list receiving per epoch what print_training prints (loss, density, pred; explain.py:148-159) and the terms it is made
+    of; size_edges / ent_edges restrict the size and entropy terms to the entries of the sub-adjacency (the only mask entries that
+    can reach the constrained result), size_off / ent_off are the complement.  density is mask_density, which keeps the
+    constrained _masked_adj in both modes (explain.py:680-683)."""
+    import torch
+    hp = hp or default_hparams()
+    dtype = dtype or torch.float
+    W = weights if isinstance(weights, dict) and "conv_w" in weights else weights_to_torch(weights, dtype=dtype)
+    n = sub_adj.shape[0]
+    adj = torch.tensor(np.asarray(sub_adj)[None], dtype=dtype)                             # explain.py:97
+    x = torch.tensor(np.asarray(sub_feat)[None], requires_grad=True, dtype=dtype)          # :98
+    mask = torch.nn.Parameter(torch.tensor(np.asarray(M0), dtype=dtype))                   # explain.py:646-652
+    feat_mask = torch.nn.Parameter(torch.zeros(x.size(-1), dtype=dtype))                   # explain.py:633-643
+    diag_mask = torch.ones(n, n, dtype=dtype) - torch.eye(n, dtype=dtype)                  # explain.py:617
+    opt, sched = build_optimizer(hp, [mask, feat_mask])
+    pred_label_t = None if graph_mode else torch.tensor(np.asarray(pred_label), dtype=dtype)
+    # explainer.zero_grad() (explain.py:138) clears the frozen model's weight gradients too: it is a sub-module
+    leaves = ([mask, feat_mask, x] + W["conv_w"] + [b for b in W["conv_b"] if b is not None] + W.get("att_w", [])
+              + [p for layer in W.get("head", ()) for p in layer] + [W["pred_w"], W["pred_b"]])
+    masked_adj = terms = None
+    for epoch in range(hp.num_epochs):                                                     # explain.py:137
+        for p in leaves:
             p.grad = None
-        if x.grad is not None:
-            x.grad = None
-        masked_adj = masked_adj_fn()                                            # explain.py:694
-        xm = x * torch.sigmoid(feat_mask)                                       # explain.py:695-707
-        ypred = _gcn_forward_torch(xm, masked_adj, W, graph_mode, bn)           # explain.py:709
-        if graph_mode:
-            res = torch.softmax(ypred[0], dim=0)                                # explain.py:711
-        else:
-            res = torch.softmax(ypred[-1, node_idx_new, :], dim=0)              # explain.py:713-714
-        pred_loss = -torch.log(res[int(gt_label)])                              # explain.py:750-753
-        m = torch.sigmoid(mask)                                                 # explain.py:756-757
-        size_loss = hp.size * torch.sum(m)                                      # explain.py:760
-        fm = torch.sigmoid(feat_mask)
-        fm_used = fm.detach()
-        feat_size_loss = hp.feat_size * torch.mean(fm)                          # explain.py:766
-        mask_ent = -m * torch.log(m) - (1 - m) * torch.log(1 - m)               # explain.py:769
-        mask_ent_loss = hp.ent * torch.mean(mask_ent)                           # explain.py:770
-        if graph_mode:
-            lap_loss = 0                                                        # explain.py:787-788
-        else:
-            D = torch.diag(torch.sum(masked_adj[0], 0))                         # explain.py:780
-            Lm = D - masked_adj[-1]                                             # explain.py:781-782
-            lap_loss = hp.lap * (pred_label_t @ Lm @ pred_label_t) / adj.numel()  # explain.py:789-793
-        loss = pred_loss + size_loss + lap_loss + mask_ent_loss + feat_size_loss  # explain.py:808
-        m_used, ent_used = m.detach(), mask_ent.detach()
-        loss.backward()                                                         # explain.py:142
-        opt.step()                                                              # explain.py:144
+        loss, masked_adj, res, terms = _epoch_loss(mask, feat_mask, adj, x, diag_mask, W, gt_label, pred_label_t, node_idx_new, hp,
+                                                   graph_mode, bn, unconstrained)
+        loss.backward()                                                                    # explain.py:142
+        opt.step()                                                                         # explain.py:144
         if sched is not None:
-            sched.step()                                                        # explain.py:145-146
-        with torch.no_grad():
-            density = torch.sum(masked_adj_fn()) / torch.sum(adj)               # explain.py:148,680-683
+            sched.step()                                                                   # explain.py:145-146
         if trace is not None:
-            # what print_training prints (explain.py:148-159) plus the terms it is made of; "edges" = restricted to the entries of
-            # the sub-adjacency (the only mask entries that can reach the result), the complement is the "off" part
             with torch.no_grad():
+                density = torch.sum(adj * _sym(mask) * diag_mask) / torch.sum(adj)         # explain.py:148,680-683
                 on = adj[0] > 0
+                m, ent = terms["m"], terms["mask_ent"]
                 trace.append(dict(loss=float(loss), density=float(density), pred=res.detach().numpy().copy(),
-                                  pred_loss=float(pred_loss), lap=float(lap_loss), feat_size=float(feat_size_loss),
-                                  size_edges=float(hp.size * torch.sum(m_used[on])), size_off=float(hp.size * torch.sum(m_used[~on])),
-                                  ent_edges=float(hp.ent * torch.sum(ent_used[on]) / adj.numel()),
-                                  ent_off=float(hp.ent * torch.sum(ent_used[~on]) / adj.numel())))
-    out = masked_adj[0].detach().numpy() * np.asarray(sub_adj, dtype=np.float64)   # explain.py:209-211
+                                  pred_loss=float(terms["pred_loss"]), lap=float(terms["lap"]), feat_size=float(terms["feat_size"]),
+                                  size=float(terms["size"]), ent=float(terms["ent"]),
+                                  size_edges=float(hp.size * torch.sum(m[on])), size_off=float(hp.size * torch.sum(m[~on])),
+                                  ent_edges=float(hp.ent * torch.sum(ent[on]) / adj.numel()),
+                                  ent_off=float(hp.ent * torch.sum(ent[~on]) / adj.numel())))
+    out = masked_adj[0].detach().numpy().astype(np.float64)
+    if not full:
+        out = out * np.asarray(sub_adj, dtype=np.float64)                                  # explain.py:209-211
     if return_feat:
-        return out, fm_used.numpy().astype(np.float64)
+        return out, terms["fm"].detach().numpy().astype(np.float64)
     return out
 
 
@@ -360,12 +427,7 @@ def grad_baseline_dense_torch(sub_adj, sub_feat, pred_label_node, node_idx_new, 
     tdt = torch.float64 if dtype == np.float64 else torch.float
     A = torch.tensor(np.asarray(sub_adj, dtype)[None], dtype=tdt, requires_grad=True)
     x = torch.tensor(np.asarray(sub_feat, dtype)[None], dtype=tdt, requires_grad=True)
-    W = weights_to_torch(weights)
-    if tdt == torch.float64:
-        W = dict(conv_w=[w.detach().double() for w in W["conv_w"]],
-                 conv_b=[None if b is None else b.detach().double() for b in W["conv_b"]],
-                 pred_w=W["pred_w"].detach().double(), pred_b=W["pred_b"].detach().double())
-    ypred = _gcn_forward_torch(x, A, W, False)
+    ypred = _gcn_forward_torch(x, A, weights_to_torch(weights, dtype=tdt), False)
     logit = torch.softmax(ypred[0, node_idx_new, :], dim=0)[int(pred_label_node)]
     loss = -torch.log(logit)
     loss.backward()

@@ -1,137 +1,16 @@
-"""att_oracle.py -- CPU restatements of Explainer.explain on an attention model (train.py / explainer_main.py --method att).
+"""att_oracle.py -- the hand-derived backward of Explainer.explain on an attention model (train.py / explainer_main.py --method att).
 TEST INFRASTRUCTURE ONLY.
 
 An attention GraphConv (models.py:62-68) scales the adjacency it is given by the unnormalised scores s = P P^T, P = H_{l-1} Wa_l,
-before the usual aggregation; every layer gets the explainer's masked adjacency (models.py:240,250,256,278-297).  Two restatements,
-built on the helpers of oracle/gnnx_oracle.py:
-  * explain_att_torch    -- line-by-line port (dense tensors, torch autograd, torch.optim); dtype=torch.float64 gives the fp64
-                            specification the kernel's single update is checked against.
+before the usual aggregation; every layer gets the explainer's masked adjacency (models.py:240,250,256,278-297).  The torch port
+(gnnx_oracle.explain_dense_torch) runs these models when the weights carry Wa1 .. WaL; here:
   * mask_grads_closed_form -- the hand-derived backward of one epoch (numpy, fp64): dL/dM and dL/dfeat_mask from the equations in
-                            DESIGN.md ("Attention models"), checked against autograd.
+                            DESIGN.md ("Attention models"), checked against autograd (tests/mask_grad_oracle.py).
 weights: the gnnx_oracle weight dict plus Wa1 .. WaL, the (in, in) att_weight matrices.
 """
 import numpy as np
 
 import gnnx_oracle as O
-from dense_oracle import _optimizer
-
-
-def att_weights_to_torch(weights, dtype=None, requires_grad=True):
-    import torch
-    dtype = dtype or torch.float
-    t = lambda a: torch.tensor(np.asarray(a), dtype=dtype, requires_grad=requires_grad)
-    W = O.weights_to_torch(weights, requires_grad)
-    W = {k: ([t(x.detach().numpy()) if x is not None else None for x in v] if isinstance(v, list) else t(v.detach().numpy()))
-         for k, v in W.items()}
-    W["att_w"] = [t(weights["Wa%d" % (l + 1)]) for l in range(len(W["conv_w"]))]
-    return W
-
-
-def gcn_forward_att_torch(x, adj, W, graph_mode, bn=False):
-    """gnnx_oracle._gcn_forward_torch with the attention of models.py:62-68 in every layer."""
-    import torch
-    import torch.nn.functional as F
-    outs = []
-    h = x
-    L = len(W["conv_w"])
-    for l in range(L):
-        x_att = torch.matmul(h, W["att_w"][l])                 # models.py:63
-        att = x_att @ x_att.permute(0, 2, 1)                   # models.py:66
-        a = adj * att                                          # models.py:68
-        y = torch.matmul(a, h)
-        y = torch.matmul(y, W["conv_w"][l])
-        if W["conv_b"][l] is not None:
-            y = y + W["conv_b"][l]
-        y = F.normalize(y, p=2, dim=2)
-        if l < L - 1:
-            y = torch.relu(y)
-            if bn:
-                y = F.batch_norm(y, None, None, None, None, True, 0.1, 1e-5)
-        outs.append(y)
-        h = y
-    if graph_mode:
-        emb = torch.cat(O.max_pool(outs), dim=1)
-        return F.linear(emb, W["pred_w"], W["pred_b"])
-    return F.linear(torch.cat(outs, dim=2), W["pred_w"], W["pred_b"])
-
-
-def model_pred_att(adj, feat, weights, bn=False, graph_mode=False):
-    """GcnEncoderNode / GcnEncoderGraph.forward on the raw adjacency (self loops included): the `pred` of the checkpoint."""
-    import torch
-    W = att_weights_to_torch(weights, requires_grad=False)
-    with torch.no_grad():
-        return gcn_forward_att_torch(torch.tensor(np.asarray(feat, np.float32)[None]), torch.tensor(np.asarray(adj, np.float32)[None]),
-                                     W, graph_mode, bn)[0].numpy()
-
-
-def _loss(W, adj, x, mask, feat_mask, diag_mask, gt_label, pred_label_t, node_idx_new, hp, graph_mode, bn):
-    """explain.py:665-808 with the attention forward: (loss, masked_adj, sigmoid(feat_mask))."""
-    import torch
-    sym = torch.sigmoid(mask)
-    sym = (sym + sym.t()) / 2
-    masked_adj = adj * sym * diag_mask
-    fm = torch.sigmoid(feat_mask)
-    ypred = gcn_forward_att_torch(x * fm, masked_adj, W, graph_mode, bn)
-    res = torch.softmax(ypred[0] if graph_mode else ypred[-1, node_idx_new, :], dim=0)
-    pred_loss = -torch.log(res[int(gt_label)])
-    m = torch.sigmoid(mask)
-    size_loss = hp.size * torch.sum(m)
-    feat_size_loss = hp.feat_size * torch.mean(fm)
-    mask_ent = -m * torch.log(m) - (1 - m) * torch.log(1 - m)
-    mask_ent_loss = hp.ent * torch.mean(mask_ent)
-    if graph_mode:
-        lap_loss = 0
-    else:
-        D = torch.diag(torch.sum(masked_adj[0], 0))
-        lap_loss = hp.lap * (pred_label_t @ (D - masked_adj[-1]) @ pred_label_t) / adj.numel()
-    return pred_loss + size_loss + lap_loss + mask_ent_loss + feat_size_loss, masked_adj, fm
-
-
-def explain_att_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0, hp=None, graph_mode=False, bn=False,
-                      dtype=None, return_feat=False):
-    """Port of Explainer.explain's optimisation (explain.py:97-146,209-211) on an attention model.  Arguments as
-    gnnx_oracle.explain_dense_torch.  Returns the (n,n) float64 masked adjacency (and sigmoid(feat_mask) as the last forward used it)."""
-    import torch
-    hp = hp or O.default_hparams()
-    dtype = dtype or torch.float
-    W = att_weights_to_torch(weights, dtype)
-    n = sub_adj.shape[0]
-    adj = torch.tensor(np.asarray(sub_adj)[None], dtype=dtype)
-    x = torch.tensor(np.asarray(sub_feat)[None], dtype=dtype, requires_grad=True)
-    mask = torch.nn.Parameter(torch.tensor(np.asarray(M0), dtype=dtype))
-    feat_mask = torch.nn.Parameter(torch.zeros(x.size(-1), dtype=dtype))
-    diag_mask = torch.ones(n, n, dtype=dtype) - torch.eye(n, dtype=dtype)
-    opt, sched = _optimizer(hp, [mask, feat_mask])
-    pred_label_t = None if graph_mode else torch.tensor(np.asarray(pred_label), dtype=dtype)
-    masked_adj = fm = None
-    for _ in range(hp.num_epochs):
-        opt.zero_grad()
-        loss, masked_adj, fm = _loss(W, adj, x, mask, feat_mask, diag_mask, gt_label, pred_label_t, node_idx_new, hp, graph_mode, bn)
-        fm = fm.detach()
-        loss.backward()
-        opt.step()
-        if sched is not None:
-            sched.step()
-    out = masked_adj[0].detach().numpy().astype(np.float64) * np.asarray(sub_adj, dtype=np.float64)
-    return (out, fm.numpy().astype(np.float64)) if return_feat else out
-
-
-def mask_grads_autograd(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M, F, hp=None, graph_mode=False, bn=False):
-    """dL/dM and dL/dfeat_mask of one epoch by torch autograd in fp64 (the reference for mask_grads_closed_form)."""
-    import torch
-    hp = hp or O.default_hparams()
-    dt = torch.float64
-    W = att_weights_to_torch(weights, dt, requires_grad=False)
-    n = sub_adj.shape[0]
-    adj = torch.tensor(np.asarray(sub_adj)[None], dtype=dt)
-    x = torch.tensor(np.asarray(sub_feat)[None], dtype=dt)
-    mask = torch.tensor(np.asarray(M), dtype=dt, requires_grad=True)
-    feat_mask = torch.tensor(np.asarray(F), dtype=dt, requires_grad=True)
-    diag_mask = torch.ones(n, n, dtype=dt) - torch.eye(n, dtype=dt)
-    pl = None if graph_mode else torch.tensor(np.asarray(pred_label), dtype=dt)
-    loss, _, _ = _loss(W, adj, x, mask, feat_mask, diag_mask, gt_label, pl, node_idx_new, hp, graph_mode, bn)
-    loss.backward()
-    return mask.grad.numpy(), feat_mask.grad.numpy()
 
 
 def _sig(z):

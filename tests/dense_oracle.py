@@ -1,12 +1,11 @@
-"""dense_oracle.py -- CPU restatements of Explainer.explain(..., unconstrained=True).  TEST INFRASTRUCTURE ONLY.
+"""dense_oracle.py -- the hand-derived restatement of Explainer.explain(..., unconstrained=True).  TEST INFRASTRUCTURE ONLY.
 
 With unconstrained=True (ExplainModule.forward, explain.py:688-692) the forward's adjacency is the DENSE mask
-sym(sigmoid(M)) * (1 - I), not multiplied by the sub-adjacency, and the features are not masked.  Two restatements, as for the
-constrained path in oracle/gnnx_oracle.py (whose helpers they reuse):
-  * explain_dense_torch  -- line-by-line port (dense tensors, torch autograd, torch.optim), bit-exact to the unmodified reference
-                            (tests/golden/unconstrained_golden.npz, tools/gen_unconstrained_golden.py); the CPU baseline.
+sym(sigmoid(M)) * (1 - I), not multiplied by the sub-adjacency, and the features are not masked.  The line-by-line torch port of
+that path is gnnx_oracle.explain_dense_torch(..., unconstrained=True), bit-exact to the unmodified reference
+(tests/golden/unconstrained_golden.npz, tools/gen_unconstrained_golden.py); here:
   * explain_closed_form  -- hand-derived forward / backward in numpy (fp64 or fp32): the specification csrc/explain_dense.cu implements.
-Both return the (n, n) float64 array the reference returns, masked_adj[0] * sub_adj (explain.py:209-211), or with full=True the whole
+It returns the (n, n) float64 array the reference returns, masked_adj[0] * sub_adj (explain.py:209-211), or with full=True the whole
 masked_adj[0] ExplainModule.forward built (the kernel's mask_dense output).
 """
 import math
@@ -27,93 +26,6 @@ def entry_classes(A):
     both = live[:, None] & live[None, :]
     cls = {"edge": off & (A != 0), "nonedge": off & (A == 0) & both, "pad": off & ~both}
     return {k: np.nonzero(v) for k, v in cls.items() if v.any()}
-
-
-def _optimizer(hp, params):
-    """utils/train_utils.py:7-23 (build_optimizer; explain.py:622)."""
-    import torch
-    if hp.opt == "adam":
-        opt = torch.optim.Adam(params, lr=hp.lr, betas=(hp.beta1, hp.beta2), eps=hp.eps)
-    elif hp.opt == "sgd":
-        opt = torch.optim.SGD(params, lr=hp.lr, momentum=0.95)
-    elif hp.opt == "rmsprop":
-        opt = torch.optim.RMSprop(params, lr=hp.lr)
-    elif hp.opt == "adagrad":
-        opt = torch.optim.Adagrad(params, lr=hp.lr)
-    else:
-        raise ValueError(hp.opt)
-    sched = None
-    if hp.opt_scheduler == "step":
-        sched = torch.optim.lr_scheduler.StepLR(opt, step_size=hp.opt_decay_step, gamma=hp.opt_decay_rate)
-    elif hp.opt_scheduler == "cos":
-        sched = torch.optim.lr_scheduler.CosineAnnealingLR(opt, T_max=hp.opt_restart)
-    return opt, sched
-
-
-def explain_dense_torch(sub_adj, sub_feat, gt_label, pred_label, node_idx_new, weights, M0, hp=None, graph_mode=False, trace=None,
-                        bn=False, full=False):
-    """Port of Explainer.explain(..., unconstrained=True) (explain.py:97-146,209-211) with ExplainModule.{forward (unconstrained
-    branch), loss, mask_density} (explain.py:680-808) inlined.  Arguments as gnnx_oracle.explain_dense_torch; M0 (n,n) float32, every
-    entry of which is a parameter here.  trace: list receiving per epoch what print_training prints (loss, density, pred) and the terms.
-    mask_density keeps the CONSTRAINED _masked_adj (explain.py:680-683).  full=True returns masked_adj[0] itself, all n^2 entries."""
-    import torch
-    hp = hp or O.default_hparams()
-    W = weights if isinstance(weights, dict) and "conv_w" in weights else O.weights_to_torch(weights)
-    n = sub_adj.shape[0]
-    adj = torch.tensor(np.asarray(sub_adj)[None], dtype=torch.float)            # explain.py:97
-    x = torch.tensor(np.asarray(sub_feat)[None], requires_grad=True, dtype=torch.float)  # :98
-    mask = torch.nn.Parameter(torch.tensor(np.asarray(M0), dtype=torch.float))  # explain.py:646-652
-    feat_mask = torch.nn.Parameter(torch.zeros(x.size(-1)))                     # explain.py:633-643
-    diag_mask = torch.ones(n, n) - torch.eye(n)                                 # explain.py:617
-    opt, sched = _optimizer(hp, [mask, feat_mask])
-    params = [mask, feat_mask] + W["conv_w"] + [b for b in W["conv_b"] if b is not None] + [W["pred_w"], W["pred_b"]]
-    pred_label_t = None if graph_mode else torch.tensor(np.asarray(pred_label), dtype=torch.float)
-
-    def constrained_adj_fn():                                                   # explain.py:665-678 (mask_density only)
-        sym = torch.sigmoid(mask)
-        sym = (sym + sym.t()) / 2
-        return adj * sym * diag_mask
-
-    masked_adj = None
-    for epoch in range(hp.num_epochs):                                          # explain.py:137
-        for p in params:
-            p.grad = None
-        if x.grad is not None:
-            x.grad = None
-        sym = torch.sigmoid(mask)                                               # explain.py:688-692
-        masked_adj = torch.unsqueeze((sym + sym.t()) / 2, 0) * diag_mask
-        ypred = O._gcn_forward_torch(x, masked_adj, W, graph_mode, bn)          # explain.py:709, raw features
-        if graph_mode:
-            res = torch.softmax(ypred[0], dim=0)                                # explain.py:711
-        else:
-            res = torch.softmax(ypred[-1, node_idx_new, :], dim=0)              # explain.py:713-714
-        pred_loss = -torch.log(res[int(gt_label)])                              # explain.py:750-753
-        m = torch.sigmoid(mask)                                                 # explain.py:756-757
-        size_loss = hp.size * torch.sum(m)                                      # explain.py:760
-        fm = torch.sigmoid(feat_mask)
-        feat_size_loss = hp.feat_size * torch.mean(fm)                          # explain.py:766
-        mask_ent = -m * torch.log(m) - (1 - m) * torch.log(1 - m)               # explain.py:769
-        mask_ent_loss = hp.ent * torch.mean(mask_ent)                           # explain.py:770
-        if graph_mode:
-            lap_loss = 0                                                        # explain.py:787-788
-        else:
-            D = torch.diag(torch.sum(masked_adj[0], 0))                         # explain.py:780
-            Lm = D - masked_adj[-1]                                             # explain.py:781-782
-            lap_loss = hp.lap * (pred_label_t @ Lm @ pred_label_t) / adj.numel()  # explain.py:789-793
-        loss = pred_loss + size_loss + lap_loss + mask_ent_loss + feat_size_loss  # explain.py:808
-        loss.backward()                                                         # explain.py:142
-        opt.step()                                                              # explain.py:144
-        if sched is not None:
-            sched.step()                                                        # explain.py:145-146
-        with torch.no_grad():
-            density = torch.sum(constrained_adj_fn()) / torch.sum(adj)          # explain.py:148,680-683
-        if trace is not None:
-            v = lambda t: float(t.detach()) if torch.is_tensor(t) else float(t)
-            trace.append(dict(loss=v(loss), density=v(density), pred=res.detach().numpy().copy(), pred_loss=v(pred_loss),
-                              lap=v(lap_loss), feat_size=v(feat_size_loss), size=v(size_loss), ent=v(mask_ent_loss)))
-    if full:
-        return masked_adj[0].detach().numpy().astype(np.float64)
-    return masked_adj[0].detach().numpy() * np.asarray(sub_adj, dtype=np.float64)   # explain.py:209-211
 
 
 def _lr_at(hp, t):

@@ -15,20 +15,12 @@ import torch
 import gnnx_oracle as O
 
 
-def _weights(weights, tdt):
-    W = O.weights_to_torch(weights)      # requires_grad like the reference's frozen sub-module
-    if tdt == torch.float64:
-        W = dict(conv_w=[w.detach().double() for w in W["conv_w"]], conv_b=[None if b is None else b.detach().double() for b in W["conv_b"]],
-                 pred_w=W["pred_w"].detach().double(), pred_b=W["pred_b"].detach().double())
-    return W
-
-
 def grad_graph_torch(adj, feat, label, weights, dtype=np.float32, return_label=False):
     """adj (n, n) 0/1 padded graph, feat (n, d) -> (n, n) float64 mask (zero off the edges)."""
     tdt = torch.float64 if dtype == np.float64 else torch.float
     A = torch.tensor(np.asarray(adj, dtype)[None], dtype=tdt, requires_grad=True)          # explain.py:97 (requires_grad: :720)
     x = torch.tensor(np.asarray(feat, dtype)[None], dtype=tdt, requires_grad=True)         # :98
-    ypred = O._gcn_forward_torch(x, A, _weights(weights, tdt), True)                       # :729
+    ypred = O._gcn_forward_torch(x, A, O.weights_to_torch(weights, dtype=tdt), True)       # :729
     label = int(label)
     if label < 0:
         label = int(np.argmax(ypred[0].detach().numpy()))

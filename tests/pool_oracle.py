@@ -1,5 +1,5 @@
-"""Graph mode's max-pool readout with its arg-max choices made visible: the torch ports of the explainer (tests/wide_oracle.py,
-tests/att_oracle.py, tests/head_oracle.py) run unchanged, with the readout of gnnx_oracle.max_pool replaced by one that can
+"""Graph mode's max-pool readout with its arg-max choices made visible: the torch port of the explainer
+(gnnx_oracle.explain_dense_torch) runs unchanged, with the readout of gnnx_oracle.max_pool replaced by one that can
 
   * record, for every epoch whose backward is used (0 .. E-2) and every pooled column, the winning row, the runner-up and their margin
     in fp32 ulps of the winner, and
@@ -13,18 +13,7 @@ near-tie flip."""
 import numpy as np
 import torch
 
-import att_oracle as AO
 import gnnx_oracle as O
-import head_oracle as HO
-import wide_oracle as WO
-
-
-def _port(weights, unconstrained):
-    if unconstrained or HO.head_layers(weights):
-        return lambda *a, **kw: HO.explain_torch(*a, unconstrained=unconstrained, **kw)
-    if "Wa1" in weights:
-        return AO.explain_att_torch
-    return WO.explain_torch
 
 
 class _Pool:
@@ -82,8 +71,8 @@ def explain_torch_pool(sub_adj, sub_feat, gt_label, weights, M0, hp=None, bn=Fal
     pool = _Pool(flips, record, hp.num_epochs)
     prev = O.set_pool(pool)
     try:
-        out, fm = _port(weights, unconstrained)(sub_adj, sub_feat, gt_label, None, 0, weights, M0, hp, graph_mode=True, bn=bn, dtype=dtype,
-                                                return_feat=True)
+        out, fm = O.explain_dense_torch(sub_adj, sub_feat, gt_label, None, 0, weights, M0, hp, graph_mode=True, bn=bn, return_feat=True,
+                                        dtype=dtype, unconstrained=unconstrained)
     finally:
         O.set_pool(prev)
     return (out, fm, pool.rec) if record else (out, fm)

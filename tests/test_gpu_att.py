@@ -1,5 +1,5 @@
 """Attention models (--method att) on the GPU: explain_var.cu's attention path through the C ABI and the drop-in Explainer, node and
-graph mode, against the port and the fp64 specification of tests/att_oracle.py."""
+graph mode, against the port (oracle/gnnx_oracle.explain_dense_torch) in fp32 and fp64."""
 import os
 import types
 
@@ -7,7 +7,6 @@ import numpy as np
 import pytest
 import torch
 
-import att_oracle as AO
 import gnnx
 import gnnx_oracle as O
 import util
@@ -31,7 +30,7 @@ def _node_setup(seed, L, bn, hid, emb, d, C, N=48, m=2):
     feat = rng.normal(size=(N, d)).astype(np.float32)
     label = rng.integers(0, C, N).astype(np.int32)
     w = random_att_model(rng, d, hid, emb, C, L)
-    pred = AO.model_pred_att(A, feat, w, bn=bn)
+    pred = O.model_pred(A, feat, w, bn=bn)
     pred_label = np.argmax(pred, 1).astype(np.int32)
     eng = gnnx.Engine(0)
     eng.set_model(w, num_layers=L, bn=bn, att=[w["Wa%d" % l] for l in range(1, L + 1)])
@@ -86,8 +85,8 @@ def test_att_nodes_match_port(case):
     for t, node in enumerate(nodes):
         A, X, gt, pl, idx = _sub(s, node)
         ohp = O.default_hparams(num_epochs=E, **over)
-        port = AO.explain_att_torch(A, X, gt, pl, idx, s.w, dense[t], ohp, bn=bn)
-        p64 = AO.explain_att_torch(A, X, gt, pl, idx, s.w, dense[t], ohp, bn=bn, dtype=torch.float64)
+        port = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[t], ohp, bn=bn)
+        p64 = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[t], ohp, bn=bn, dtype=torch.float64)
         tol = max(1e-4, 3 * O.rel_l2(p64, port))
         err = O.rel_l2(plan.dense_of(t, out), port)
         assert err <= tol, (node, err, tol)
@@ -107,7 +106,7 @@ def test_att_one_update_matches_fp64_spec(seed, L, bn, hid, d):
     s.eng.explain_nodes_host(s.eng.make_hparams(num_epochs=2), m0, out, fm)
     for t, node in enumerate(nodes):
         A, X, gt, pl, idx = _sub(s, node)
-        ref, f1 = AO.explain_att_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, dtype=torch.float64,
+        ref, f1 = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, dtype=torch.float64,
                                        return_feat=True)
         assert O.rel_l2(plan.dense_of(t, out), ref) <= 1e-5, node
         assert np.abs(fm[t] - f1).max() <= 1e-5, node   # the feature mask after the one update
@@ -125,8 +124,8 @@ def test_att_large_subgraph_deterministic_and_order_free():
     s.eng.explain_nodes_host(s.eng.make_hparams(num_epochs=5), m0, out)
     A, X, gt, pl, idx = _sub(s, hub)
     ohp = O.default_hparams(num_epochs=5)
-    port = AO.explain_att_torch(A, X, gt, pl, idx, s.w, dense[0], ohp)
-    p64 = AO.explain_att_torch(A, X, gt, pl, idx, s.w, dense[0], ohp, dtype=torch.float64)
+    port = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[0], ohp)
+    p64 = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[0], ohp, dtype=torch.float64)
     assert O.rel_l2(plan.dense_of(0, out), port) <= max(1e-4, 3 * O.rel_l2(p64, port))
     # determinism and independence of the batch order (Philox init: keyed by node and slot)
     nodes = [3, 17, hub, 120, 999]
@@ -230,8 +229,8 @@ def test_explainer_dropin_node_mode(tmp_path, capsys, L, bn):
         A, X, gt, pl, idx = _sub(s, node)
         n = A.shape[0]
         M0 = O.draw_m0(n)
-        port = AO.explain_att_torch(A, X, s.label[node], pl, idx, s.w, M0, O.default_hparams(num_epochs=20), bn=bn)
-        p64 = AO.explain_att_torch(A, X, s.label[node], pl, idx, s.w, M0, O.default_hparams(num_epochs=20), bn=bn, dtype=torch.float64)
+        port = O.explain_dense_torch(A, X, s.label[node], pl, idx, s.w, M0, O.default_hparams(num_epochs=20), bn=bn)
+        p64 = O.explain_dense_torch(A, X, s.label[node], pl, idx, s.w, M0, O.default_hparams(num_epochs=20), bn=bn, dtype=torch.float64)
         assert O.rel_l2(got, port) <= max(1e-4, 3 * O.rel_l2(p64, port)), node
     printed = capsys.readouterr().out
     assert "trace is not built for attention models" in printed and "Saved adjacency matrix to" in printed
@@ -262,8 +261,8 @@ def test_explainer_dropin_graph_mode(tmp_path, capsys):
     for g, masked in zip(gids, got):
         M0 = O.draw_m0(n)
         A = np.asarray(gg["adj"][g], np.float64)
-        port = AO.explain_att_torch(A, gg["feat"][g], label[g], None, 0, w, M0, O.default_hparams(num_epochs=20), graph_mode=True)
-        p64 = AO.explain_att_torch(A, gg["feat"][g], label[g], None, 0, w, M0, O.default_hparams(num_epochs=20), graph_mode=True,
+        port = O.explain_dense_torch(A, gg["feat"][g], label[g], None, 0, w, M0, O.default_hparams(num_epochs=20), graph_mode=True)
+        p64 = O.explain_dense_torch(A, gg["feat"][g], label[g], None, 0, w, M0, O.default_hparams(num_epochs=20), graph_mode=True,
                                    dtype=torch.float64)
         ei, ej = np.nonzero(A)
         assert masked.shape == (n, n)

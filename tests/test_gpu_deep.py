@@ -1,7 +1,7 @@
 """GPU (-m gpu): GCNs with five to seven graph-convolution layers (num_gc_layers 5 .. 7, n_hops = num_gc_layers) on the model-variant
 kernel (explain_var.cu), the unconstrained kernel (explain_dense.cu) and the model forward (forward.cu), through the C ABI, the drop-in
 Explainer and gnnx.dist, node and graph mode: against the masks the unmodified reference returned (tests/golden/deep_golden.npz) and
-against the torch ports of tests/wide_oracle.py and tests/att_oracle.py in fp32 and fp64."""
+against the torch port (oracle/gnnx_oracle.explain_dense_torch) in fp32 and fp64."""
 import os
 import types
 
@@ -9,12 +9,9 @@ import numpy as np
 import pytest
 import torch
 
-import att_oracle as AO
-import dense_oracle as D
 import gnnx
 import gnnx_oracle as O
 import util
-import wide_oracle as WO
 from gnnx import _abi
 from test_oracle_deep import GOLDEN, case_weights, golden_cases
 
@@ -41,18 +38,6 @@ def _att_list(w, L):
     return [w["Wa%d" % l] for l in range(1, L + 1)] if "Wa1" in w else None
 
 
-def _port(w):
-    return AO.explain_att_torch if "Wa1" in w else WO.explain_torch
-
-
-def _model_pred(A, feat, w, bn):
-    if "Wa1" in w:
-        return AO.model_pred_att(A, feat, w, bn=bn)
-    with torch.no_grad():
-        return O._gcn_forward_torch(torch.tensor(feat[None]), torch.tensor(A[None], dtype=torch.float), O.weights_to_torch(w, False),
-                                    False, bn=bn)[0].numpy()
-
-
 def _node_setup(seed, L, bn, att, hid, emb, d, C, N=48, m=2):
     import networkx as nx
     rng = np.random.default_rng(seed)
@@ -61,7 +46,7 @@ def _node_setup(seed, L, bn, att, hid, emb, d, C, N=48, m=2):
     feat = rng.normal(size=(N, d)).astype(np.float32)
     label = rng.integers(0, C, N).astype(np.int32)
     w = random_model(rng, d, hid, emb, C, L, att)
-    pred = _model_pred(A, feat, w, bn)
+    pred = O.model_pred(A, feat, w, bn=bn)
     pred_label = np.argmax(pred, 1).astype(np.int32)
     eng = gnnx.Engine(0)
     eng.set_model(w, num_layers=L, bn=bn, att=_att_list(w, L))
@@ -111,8 +96,8 @@ def _ohp(E, opt="adam", sched="none"):
 
 def _check(got, fm, w, port_args, port_kw):
     """Edge mask within max(1e-4, 3 x the port's fp32 / fp64 distance); feature mask within max(1e-4, 3 x the same distance on it)."""
-    port, f32 = _port(w)(*port_args, return_feat=True, **port_kw)
-    p64, f64 = _port(w)(*port_args, return_feat=True, dtype=torch.float64, **port_kw)
+    port, f32 = O.explain_dense_torch(*port_args, return_feat=True, **port_kw)
+    p64, f64 = O.explain_dense_torch(*port_args, return_feat=True, dtype=torch.float64, **port_kw)
     tol = max(1e-4, 3 * O.rel_l2(p64, port))
     err = O.rel_l2(got, port)
     assert err <= tol, ("edge mask", err, tol)
@@ -197,8 +182,9 @@ def test_deep_one_update_matches_fp64_port(case):
     s.eng.close()
     for t, node in enumerate(nodes):
         A, X, gt, pl, idx = _sub(s, node)
-        ref, f1 = _port(s.w)(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, dtype=torch.float64, return_feat=True)
-        p32, f32 = _port(s.w)(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, return_feat=True)
+        ref, f1 = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, dtype=torch.float64,
+                                        return_feat=True)
+        p32, f32 = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, return_feat=True)
         assert O.rel_l2(plan.dense_of(t, out), ref) <= max(1e-5, 3 * O.rel_l2(p32, ref)), node
         assert np.abs(fm[t] - f1).max() <= max(1e-5, 3 * float(np.abs(f32 - f1).max())), node
     adj, feat, label, w, eng = _graph_setup(seed + 10, L, bn, att, hid, emb, d, 3)
@@ -213,8 +199,8 @@ def test_deep_one_update_matches_fp64_port(case):
     eng.close()
     for t, g in enumerate(gids):
         args = (np.asarray(adj[g], np.float64), feat[g], int(label[g]), None, 0, w, dense[g], O.default_hparams(num_epochs=2))
-        ref, f1 = _port(w)(*args, graph_mode=True, bn=bn, dtype=torch.float64, return_feat=True)
-        p32, f32 = _port(w)(*args, graph_mode=True, bn=bn, return_feat=True)
+        ref, f1 = O.explain_dense_torch(*args, graph_mode=True, bn=bn, dtype=torch.float64, return_feat=True)
+        p32, f32 = O.explain_dense_torch(*args, graph_mode=True, bn=bn, return_feat=True)
         assert O.rel_l2(out[edge_off[t]:edge_off[t + 1]], ref[rc[g]]) <= max(1e-5, 3 * O.rel_l2(p32[rc[g]], ref[rc[g]])), g
         assert np.abs(fm[t] - f1).max() <= max(1e-5, 3 * float(np.abs(f32 - f1).max())), g
 
@@ -285,7 +271,8 @@ def test_deep_unconstrained_matches_port(L):
     for t, v in enumerate(nodes):
         idx, srp, scol, X, lab, nbrs = O.extract_neighborhood(fx.rowptr, fx.col, fx.feat, fx.label, v, L)
         A = O.dense_from_csr(srp, scol); ei, ej = np.nonzero(A)
-        port = D.explain_dense_torch(A, X, int(lab[idx]), fx.pred_label[nbrs], idx, Wn, m0[t], hp=O.default_hparams(num_epochs=E), bn=L == 7)
+        port = O.explain_dense_torch(A, X, int(lab[idx]), fx.pred_label[nbrs], idx, Wn, m0[t], hp=O.default_hparams(num_epochs=E),
+                                     bn=L == 7, unconstrained=True)
         assert util.rel_l2(out[plan.edge_off[t]:plan.edge_off[t + 1]], port[ei, ej]) <= 1e-4, (L, v)
     eng = gnnx.Engine(0)
     eng.set_model(Wg, num_layers=L, bn=L == 5)
@@ -299,8 +286,8 @@ def test_deep_unconstrained_matches_port(L):
     eng.close()
     for t, g in enumerate(gids):
         A = GG["adj"][g].astype(np.float64); ei, ej = np.nonzero(A)
-        port = D.explain_dense_torch(A, GG["feat"][g], int(GG["label"][g]), None, 0, Wg, m0[t], hp=O.default_hparams(num_epochs=E),
-                                     graph_mode=True, bn=L == 5)
+        port = O.explain_dense_torch(A, GG["feat"][g], int(GG["label"][g]), None, 0, Wg, m0[t], hp=O.default_hparams(num_epochs=E),
+                                     graph_mode=True, bn=L == 5, unconstrained=True)
         assert util.rel_l2(out[edge_off[t]:edge_off[t + 1]], port[ei, ej]) <= 1e-4, (L, g)
 
 
@@ -385,8 +372,8 @@ def test_explainer_dropin_node_mode(tmp_path, capsys, hid, emb):
         n = A.shape[0]
         M0 = O.draw_m0(n)
         hp = O.default_hparams(num_epochs=20)
-        port = WO.explain_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True)
-        p64 = WO.explain_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True, dtype=torch.float64)
+        port = O.explain_dense_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True)
+        p64 = O.explain_dense_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True, dtype=torch.float64)
         assert O.rel_l2(got, port) <= max(1e-4, 3 * O.rel_l2(p64, port)), node
     printed = capsys.readouterr().out
     assert "trace is not built for --bn / num_gc_layers != 3" in printed and "Saved adjacency matrix to" in printed
@@ -413,8 +400,8 @@ def test_explainer_dropin_graph_mode(tmp_path, capsys):
         M0 = O.draw_m0(n)
         A = np.asarray(adj[g], np.float64)
         hp = O.default_hparams(num_epochs=20)
-        port = WO.explain_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True)
-        p64 = WO.explain_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True, dtype=torch.float64)
+        port = O.explain_dense_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True)
+        p64 = O.explain_dense_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True, dtype=torch.float64)
         ei, ej = np.nonzero(A)
         assert masked.shape == (n, n)
         assert O.rel_l2(masked[ei, ej], port[ei, ej]) <= max(1e-4, 3 * O.rel_l2(p64[ei, ej], port[ei, ej])), g

@@ -18,7 +18,6 @@ import gnnx
 from gnnx import _abi
 import dense_oracle as D
 import gnnx_oracle as O
-import head_oracle as HO
 import util
 from test_gpu_unconstrained import _args, _bench, _load, _random_model, graph_engine, graph_weights, run, run_graphs, run_nodes
 
@@ -160,11 +159,8 @@ class Task:
 
     def port(self, hp):
         """The fp32 line-by-line port's whole mask after hp.num_epochs - 1 updates."""
-        if "head" in self.W:
-            return HO.explain_torch(self.A, self.X, self.gt, self.y, self.idx, self.W, self.M0, hp=hp, graph_mode=self.graph, bn=self.bn,
-                                    unconstrained=True, full=True)
-        return D.explain_dense_torch(self.A, self.X, self.gt, self.y, self.idx, self.W, self.M0, hp=hp, graph_mode=self.graph, bn=self.bn,
-                                     full=True)
+        return O.explain_dense_torch(self.A, self.X, self.gt, self.y, self.idx, self.W, self.M0, hp=hp, graph_mode=self.graph, bn=self.bn,
+                                     full=True, unconstrained=True)
 
 
 def compare_to_closed_form(gpu, cf, port, A, what, bad, report):

@@ -11,7 +11,6 @@ import numpy as np
 import pytest
 import torch
 
-import att_oracle as AO
 import dense_oracle as DO
 import gnnx
 import gnnx_oracle as O
@@ -377,10 +376,10 @@ def _port(cs, sub, X, gt, pl, idx, M0, E, path):
     """(fp32 port, its fp64 restatement) of the optimisation on the reference's sub_adj, diagonal included."""
     hp = O.default_hparams(num_epochs=E)
     if path == "att":
-        return (AO.explain_att_torch(sub, X, gt, pl, idx, cs.weights, M0, hp, bn=cs.bn),
-                AO.explain_att_torch(sub, X, gt, pl, idx, cs.weights, M0, hp, bn=cs.bn, dtype=torch.float64))
+        return (O.explain_dense_torch(sub, X, gt, pl, idx, cs.weights, M0, hp, bn=cs.bn),
+                O.explain_dense_torch(sub, X, gt, pl, idx, cs.weights, M0, hp, bn=cs.bn, dtype=torch.float64))
     if path == "unconstrained":
-        return (DO.explain_dense_torch(sub, X, gt, pl, idx, cs.weights, M0, hp, bn=cs.bn),
+        return (O.explain_dense_torch(sub, X, gt, pl, idx, cs.weights, M0, hp, bn=cs.bn, unconstrained=True),
                 DO.explain_closed_form(sub, X, gt, pl, idx, cs.weights, M0, hp, bn=cs.bn))
     return (O.explain_dense_torch(sub, X, gt, pl, idx, cs.weights, M0, hp=hp, bn=cs.bn),
             O.explain_closed_form(sub, X, gt, pl, idx, cs.weights, M0, hp=hp, bn=cs.bn))
@@ -450,7 +449,7 @@ def test_self_loop_trace_density_matches_port(unconstrained):
         tr = []
         args = (sub, cs.feat[nbrs], cs.label[node], cs.pred_label[nbrs], idx, cs.weights, dense[t])
         if unconstrained:
-            DO.explain_dense_torch(*args, hp=O.default_hparams(num_epochs=E), trace=tr)
+            O.explain_dense_torch(*args, hp=O.default_hparams(num_epochs=E), trace=tr, unconstrained=True)
         else:
             O.explain_dense_torch(*args, hp=O.default_hparams(num_epochs=E), trace=tr)
         want = np.array([e["density"] for e in tr])

@@ -1,6 +1,6 @@
 """GPU (-m gpu): models with an MLP prediction head (pred_hidden_dims, models.py:193-207) on the model-variant kernel (explain_var.cu), the
 unconstrained kernel (explain_dense.cu) and the model forward (forward.cu), through the C ABI and the drop-in Explainer, node and graph
-mode: against the torch port of tests/head_oracle.py in fp32 and fp64."""
+mode: against the torch port (oracle/gnnx_oracle.explain_dense_torch) in fp32 and fp64."""
 import types
 
 import numpy as np
@@ -9,7 +9,6 @@ import torch
 
 import gnnx
 import gnnx_oracle as O
-import head_oracle as HO
 from gnnx import _abi
 import util
 from test_gpu_deep import GG, _hp, _m0, _ohp, random_model
@@ -44,7 +43,7 @@ def _node_setup(seed, L, bn, att, hid, emb, d, C, widths, N=48, m=2):
     feat = rng.normal(size=(N, d)).astype(np.float32)
     label = rng.integers(0, C, N).astype(np.int32)
     w = head_model(rng, d, hid, emb, C, L, widths, att)
-    pred = HO.model_pred(A, feat, w, bn=bn)
+    pred = O.model_pred(A, feat, w, bn=bn)
     pred_label = np.argmax(pred, 1).astype(np.int32)
     eng = gnnx.Engine(0)
     _set(eng, w, L, bn)
@@ -72,8 +71,8 @@ def _sub(s, node):
 
 def _check(got, fm, port_args, port_kw):
     """Edge mask within max(1e-4, 3 x the port's fp32 / fp64 distance); feature mask likewise."""
-    p32, f32 = HO.explain_torch(*port_args, return_feat=True, **port_kw)
-    p64, f64 = HO.explain_torch(*port_args, return_feat=True, dtype=torch.float64, **port_kw)
+    p32, f32 = O.explain_dense_torch(*port_args, return_feat=True, **port_kw)
+    p64, f64 = O.explain_dense_torch(*port_args, return_feat=True, dtype=torch.float64, **port_kw)
     tol = max(1e-4, 3 * O.rel_l2(p64, p32))
     err = O.rel_l2(got, p32)
     assert err <= tol, ("edge mask", err, tol)
@@ -155,7 +154,7 @@ def test_head_one_update_matches_fp64_port(graph):
         s.eng.close()
         for t, node in enumerate(nodes):
             A, X, gt, pl, idx = _sub(s, node)
-            ref, f1 = HO.explain_torch(A, X, gt, pl, idx, s.w, dense[t], hp, bn=True, dtype=torch.float64, return_feat=True)
+            ref, f1 = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[t], hp, bn=True, dtype=torch.float64, return_feat=True)
             assert O.rel_l2(plan.dense_of(t, out), ref) <= 1e-5, node
             assert np.abs(fm[t] - f1).max() <= 1e-5, node
         return
@@ -170,8 +169,8 @@ def test_head_one_update_matches_fp64_port(graph):
     eng.explain_graphs_host(eng.make_hparams(num_epochs=2), np.concatenate([dense[g][rc[g]] for g in gids]).astype(np.float32), out, fm)
     eng.close()
     for t, g in enumerate(gids):
-        ref, f1 = HO.explain_torch(np.asarray(adj[g], np.float64), feat[g], int(label[g]), None, 0, w, dense[g], hp, graph_mode=True, bn=True,
-                                   dtype=torch.float64, return_feat=True)
+        ref, f1 = O.explain_dense_torch(np.asarray(adj[g], np.float64), feat[g], int(label[g]), None, 0, w, dense[g], hp, graph_mode=True,
+                                        bn=True, dtype=torch.float64, return_feat=True)
         assert O.rel_l2(out[edge_off[t]:edge_off[t + 1]], ref[rc[g]]) <= 1e-5, g
         assert np.abs(fm[t] - f1).max() <= 1e-5, g
 

@@ -11,12 +11,10 @@ import numpy as np
 import pytest
 import torch
 
-import att_oracle as AO
 import dense_oracle as D
 import gnnx
 import gnnx_oracle as O
 import util
-import wide_oracle as WO
 from gnnx import _abi
 from test_oracle_att import random_att_model
 from test_oracle_hparams import HSETS, case_hparams, golden, gx_over
@@ -175,11 +173,11 @@ def check_port(got, fm, port, hset, E):
 
 
 def wide_port(A, X, gt, pl, idx, w, M0, graph_mode=False, bn=False):
-    return lambda hp, dt: WO.explain_torch(A, X, gt, pl, idx, w, M0, hp=hp, graph_mode=graph_mode, bn=bn, dtype=dt, return_feat=True)
+    return lambda hp, dt: O.explain_dense_torch(A, X, gt, pl, idx, w, M0, hp=hp, graph_mode=graph_mode, bn=bn, dtype=dt, return_feat=True)
 
 
 def att_port(A, X, gt, pl, idx, w, M0, graph_mode=False, bn=False):
-    return lambda hp, dt: AO.explain_att_torch(A, X, gt, pl, idx, w, M0, hp=hp, graph_mode=graph_mode, bn=bn, dtype=dt, return_feat=True)
+    return lambda hp, dt: O.explain_dense_torch(A, X, gt, pl, idx, w, M0, hp=hp, graph_mode=graph_mode, bn=bn, dtype=dt, return_feat=True)
 
 
 E_SET = 20
@@ -256,7 +254,7 @@ def test_sets_on_attention_kernel(hset):
     rowptr, col = O.csr_from_edges(48, np.array(nx.barabasi_albert_graph(48, 2, seed=31).edges(), dtype=np.int64))
     feat = rng.normal(size=(48, 10)).astype(np.float32)
     label = rng.integers(0, 3, 48).astype(np.int32)
-    pred_label = np.argmax(AO.model_pred_att(O.dense_from_csr(rowptr, col), feat, w), 1).astype(np.int32)
+    pred_label = np.argmax(O.model_pred(O.dense_from_csr(rowptr, col), feat, w), 1).astype(np.int32)
     eng = gnnx.Engine(0)
     eng.set_model(w, num_layers=3, att=att)
     eng.set_graph_csr(rowptr, col, feat, label, pred_label)
@@ -299,7 +297,7 @@ def _dense_run(graphs, hp_gx, seeds_or_gids, eng, plan=None):
 
 @pytest.mark.parametrize("hset", list(HSETS))
 def test_sets_on_dense_kernel(hset):
-    """unconstrained=True: the edge masks against dense_oracle's port within max(1e-4, 3 x its distance to the fp64 closed form)."""
+    """unconstrained=True: the edge masks against the port within max(1e-4, 3 x its distance to the fp64 closed form)."""
     hp = O.default_hparams(num_epochs=E_SET, **HSETS[hset])
     fx = util.load_fixture("rand")
     eng = util.make_engine(fx)
@@ -321,11 +319,11 @@ def test_sets_on_dense_kernel(hset):
         cases.append((outs[t], (GG["adj"][g].astype(np.float64), GG["feat"][g], int(GG["label"][g]), None, 0, GW, m0[t]), True))
     for got, args, graph_mode in cases:
         ei, ej = np.nonzero(args[0])
-        port = D.explain_dense_torch(*args, hp=hp, graph_mode=graph_mode)[ei, ej]
+        port = O.explain_dense_torch(*args, hp=hp, graph_mode=graph_mode, unconstrained=True)[ei, ej]
         cf = D.explain_closed_form(*args, hp=hp, graph_mode=graph_mode)[ei, ej]
         tol = max(1e-4, 3 * O.rel_l2(cf, port))
         assert O.rel_l2(got, port) <= tol, (hset, graph_mode, O.rel_l2(got, port), tol)
-        base = D.explain_dense_torch(*args, hp=O.default_hparams(num_epochs=E_SET), graph_mode=graph_mode)[ei, ej]
+        base = O.explain_dense_torch(*args, hp=O.default_hparams(num_epochs=E_SET), graph_mode=graph_mode, unconstrained=True)[ei, ej]
         assert O.rel_l2(base, port) > 10 * tol, (hset, graph_mode)
 
 
@@ -352,7 +350,7 @@ def _node_case(path):
         rowptr, col = O.csr_from_edges(48, np.array(nx.barabasi_albert_graph(48, 2, seed=32).edges(), dtype=np.int64))
         feat = rng.normal(size=(48, 10)).astype(np.float32)
         label = rng.integers(0, 3, 48).astype(np.int32)
-        pl = np.argmax(AO.model_pred_att(O.dense_from_csr(rowptr, col), feat, w), 1).astype(np.int32)
+        pl = np.argmax(O.model_pred(O.dense_from_csr(rowptr, col), feat, w), 1).astype(np.int32)
         eng = gnnx.Engine(0)
         eng.set_model(w, num_layers=3, att=[w["Wa%d" % l] for l in range(1, 4)])
         eng.set_graph_csr(rowptr, col, feat, label, pl)
@@ -447,9 +445,9 @@ def test_one_update_matches_fp64_nodes(path, hset):
         if path == "dense":
             ref, f1 = D.explain_closed_form(*args, hp=hp), None
         elif path == "att":
-            ref, f1 = AO.explain_att_torch(*args, hp=hp, dtype=torch.float64, return_feat=True)
+            ref, f1 = O.explain_dense_torch(*args, hp=hp, dtype=torch.float64, return_feat=True)
         elif path in ("variant", "wide"):
-            ref, f1 = WO.explain_torch(*args, hp=hp, bn=bn, dtype=torch.float64, return_feat=True)
+            ref, f1 = O.explain_dense_torch(*args, hp=hp, bn=bn, dtype=torch.float64, return_feat=True)
         else:
             ref = O.explain_closed_form(*args, hp=hp)
             _, st = O.explain_closed_form(*args, hp=O.default_hparams(num_epochs=1, **HSETS[hset]), return_state=True)
@@ -480,9 +478,9 @@ def test_one_update_matches_fp64_graphs(path, hset):
         if path == "dense":
             ref, f1 = D.explain_closed_form(*args, hp=hp, graph_mode=True), None
         elif path == "att":
-            ref, f1 = AO.explain_att_torch(*args, hp=hp, graph_mode=True, dtype=torch.float64, return_feat=True)
+            ref, f1 = O.explain_dense_torch(*args, hp=hp, graph_mode=True, dtype=torch.float64, return_feat=True)
         elif path in ("variant", "wide"):
-            ref, f1 = WO.explain_torch(*args, hp=hp, graph_mode=True, bn=bn, dtype=torch.float64, return_feat=True)
+            ref, f1 = O.explain_dense_torch(*args, hp=hp, graph_mode=True, bn=bn, dtype=torch.float64, return_feat=True)
         else:
             ref = O.explain_closed_form(*args, hp=hp, graph_mode=True)
             _, st = O.explain_closed_form(*args, hp=O.default_hparams(num_epochs=1, **HSETS[hset]), graph_mode=True, return_state=True)

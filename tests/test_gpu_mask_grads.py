@@ -51,12 +51,12 @@ def _logit(p):
 
 # ------------------------------------------------------------------------------------------------ problems and the oracle
 class Problem:
-    """One task (node or graph) with its oracle.  model: dict(bn, att, head, unconstrained) flags of mask_grads."""
+    """One task (node or graph) with its oracle.  model: dict(bn, unconstrained) flags of mask_grads (the weights carry the model)."""
 
     def __init__(self, A, X, gt, pl, idx, w, graph_mode, **model):
         self.A, self.X, self.gt, self.pl, self.idx, self.w = np.asarray(A, np.float64), np.asarray(X), int(gt), pl, int(idx), w
         self.graph_mode = graph_mode
-        self.model = {**dict(bn=False, att=False, head=False, unconstrained=False), **model}
+        self.model = {**dict(bn=False, unconstrained=False), **model}
         self.n, self.d = self.A.shape[0], self.X.shape[1]
 
     def grads(self, M, F):
@@ -446,14 +446,12 @@ def _model(tag, seed, d_default=10):
         from test_oracle_att import random_att_model
         w = random_att_model(rng, d, hid, emb, C, L)
         kw["att"] = [w["Wa%d" % (l + 1)] for l in range(L)]
-        flags["att"] = True
     if tag.startswith("head"):
         dims = [50] if tag == "head50" else [256, 7]
         head = _head(rng, hid * (L - 1) + emb, dims)
         w["head"] = head
         w["Wp"] = (rng.normal(size=(C, dims[-1])) * 0.5).astype(np.float32)
         kw["head"] = head
-        flags["head"] = True
     return w, L, bn, kw, flags, d
 
 

@@ -20,7 +20,6 @@ import torch
 import gnnx
 from gnnx import _abi
 import gnnx_oracle as O
-import head_oracle as HO
 import util
 
 pytestmark = pytest.mark.gpu
@@ -126,8 +125,8 @@ def seg(a, off, t):
 
 def port_check(got, fm, args, kw):
     """Edge mask within max(1e-4, 3 x the fp32 / fp64 distance of the torch port), the feature mask likewise."""
-    p32, f32 = HO.explain_torch(*args, return_feat=True, **kw)
-    p64, f64 = HO.explain_torch(*args, return_feat=True, dtype=torch.float64, **kw)
+    p32, f32 = O.explain_dense_torch(*args, return_feat=True, **kw)
+    p64, f64 = O.explain_dense_torch(*args, return_feat=True, dtype=torch.float64, **kw)
     tol = max(1e-4, 3 * O.rel_l2(p64, p32))
     err = O.rel_l2(got, p32)
     assert err <= tol, ("edge mask", err, tol)
@@ -408,7 +407,7 @@ def test_variant_kernel_node_queue_past_its_grid(name, sms):
     feat = rng.normal(size=(N, d)).astype(np.float32)
     label = rng.integers(0, C, N).astype(np.int32)
     w = random_model(rng, d, hid, emb, C, L, att, head)
-    pred_label = np.argmax(HO.model_pred(O.dense_from_csr(rowptr, col), feat, w, bn=bn), 1).astype(np.int32)
+    pred_label = np.argmax(O.model_pred(O.dense_from_csr(rowptr, col), feat, w, bn=bn), 1).astype(np.int32)
     comps = [component(rowptr, col, feat, label, pred_label, v, L) for v in VAR_ROOTS]
     K = 520
     g = union(comps, K)

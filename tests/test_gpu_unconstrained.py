@@ -237,7 +237,7 @@ def test_models_and_optimisers_match_port(case):
     for t, v in enumerate(nodes):
         idx, srp, scol, X, lab, nbrs = O.extract_neighborhood(fx.rowptr, fx.col, fx.feat, fx.label, v, L)
         A = O.dense_from_csr(srp, scol); ei, ej = np.nonzero(A)
-        port = D.explain_dense_torch(A, X, int(lab[idx]), fx.pred_label[nbrs], idx, Wn, m0[t], hp=hp_cf, bn=bn)
+        port = O.explain_dense_torch(A, X, int(lab[idx]), fx.pred_label[nbrs], idx, Wn, m0[t], hp=hp_cf, bn=bn, unconstrained=True)
         assert util.rel_l2(seg(out, plan.edge_off, t), port[ei, ej]) <= 1e-4, (case, v)
     eng.close()
     eng = graph_engine(Wg, L, bn)
@@ -246,7 +246,8 @@ def test_models_and_optimisers_match_port(case):
     edge_off, (out, _, _, _) = run_graphs(eng, gids, eng.make_hparams(num_epochs=E, **gx_opt), m0)
     for t, g in enumerate(gids):
         A = GG["adj"][g].astype(np.float64); ei, ej = np.nonzero(A)
-        port = D.explain_dense_torch(A, GG["feat"][g], int(GG["label"][g]), None, 0, Wg, m0[t], hp=hp_cf, graph_mode=True, bn=bn)
+        port = O.explain_dense_torch(A, GG["feat"][g], int(GG["label"][g]), None, 0, Wg, m0[t], hp=hp_cf, graph_mode=True, bn=bn,
+                                     unconstrained=True)
         assert util.rel_l2(seg(out, edge_off, t), port[ei, ej]) <= 1e-4, (case, g)
     eng.close()
 
@@ -279,7 +280,7 @@ def test_large_subgraph_and_refusals():
     out, _, _, _ = run_nodes(eng, plan, eng.make_hparams(num_epochs=3), m0)
     idx, srp, scol, X, lab, nbrs = O.extract_neighborhood(rowptr, col, feat, label, node, 3)
     A = O.dense_from_csr(srp, scol); ei, ej = np.nonzero(A)
-    port = D.explain_dense_torch(A, X, int(lab[idx]), pl[nbrs], idx, W, m0[0], hp=O.default_hparams(num_epochs=3))
+    port = O.explain_dense_torch(A, X, int(lab[idx]), pl[nbrs], idx, W, m0[0], hp=O.default_hparams(num_epochs=3), unconstrained=True)
     assert util.rel_l2(out[:plan.total_edges], port[ei, ej]) <= 1e-4
     for over in (dict(init=_abi.GX_INIT_STATE), dict(mask_act=1)):
         with pytest.raises(_abi.GnnxError) as e:

@@ -1,5 +1,5 @@
 """GPU (-m gpu): inputs wider than 128 features (explain_var.cu's wide path, 129 <= d <= 4096) through the C ABI, the drop-in Explainer
-and gnnx.dist, node and graph mode, against the torch port of tests/wide_oracle.py in fp32 and fp64."""
+and gnnx.dist, node and graph mode, against the torch port (oracle/gnnx_oracle.explain_dense_torch) in fp32 and fp64."""
 import os
 import types
 
@@ -10,7 +10,6 @@ import torch
 import gnnx
 import gnnx_oracle as O
 import util
-import wide_oracle as WO
 from gnnx import _abi
 
 pytestmark = pytest.mark.gpu
@@ -77,8 +76,8 @@ def _ohp(E, opt="adam", sched="none"):
 
 def _check(got, fm, port_args, port_kw):
     """Edge mask within max(1e-4, 3 x the port's fp32 / fp64 distance); feature mask within max(1e-4, 3 x the same distance on it)."""
-    port, f32 = WO.explain_torch(*port_args, return_feat=True, **port_kw)
-    p64, f64 = WO.explain_torch(*port_args, return_feat=True, dtype=torch.float64, **port_kw)
+    port, f32 = O.explain_dense_torch(*port_args, return_feat=True, **port_kw)
+    p64, f64 = O.explain_dense_torch(*port_args, return_feat=True, dtype=torch.float64, **port_kw)
     tol = max(1e-4, 3 * O.rel_l2(p64, port))
     err = O.rel_l2(got, port)
     assert err <= tol, ("edge mask", err, tol)
@@ -171,7 +170,7 @@ def test_wide_one_update_matches_fp64_port():
     s.eng.close()
     for t, node in enumerate(nodes):
         A, X, gt, pl, idx = _sub(s, node)
-        ref, f1 = WO.explain_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=True, dtype=torch.float64,
+        ref, f1 = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=True, dtype=torch.float64,
                                    return_feat=True)
         assert O.rel_l2(plan.dense_of(t, out), ref) <= 1e-5, node
         assert np.abs(fm[t] - f1).max() <= 1e-5, node
@@ -186,7 +185,7 @@ def test_wide_one_update_matches_fp64_port():
     eng.explain_graphs_host(eng.make_hparams(num_epochs=2), np.concatenate([dense[g][rc[g]] for g in gids]).astype(np.float32), out, fm)
     eng.close()
     for t, g in enumerate(gids):
-        ref, f1 = WO.explain_torch(np.asarray(adj[g], np.float64), feat[g], int(label[g]), None, 0, w, dense[g],
+        ref, f1 = O.explain_dense_torch(np.asarray(adj[g], np.float64), feat[g], int(label[g]), None, 0, w, dense[g],
                                    O.default_hparams(num_epochs=2), graph_mode=True, bn=True, dtype=torch.float64, return_feat=True)
         assert O.rel_l2(out[edge_off[t]:edge_off[t + 1]], ref[rc[g]]) <= 1e-5, g
         assert np.abs(fm[t] - f1).max() <= 1e-5, g
@@ -341,8 +340,8 @@ def test_explainer_dropin_node_mode(tmp_path, capsys):
         n = A.shape[0]
         M0 = O.draw_m0(n)
         hp = O.default_hparams(num_epochs=20)
-        port = WO.explain_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True)
-        p64 = WO.explain_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True, dtype=torch.float64)
+        port = O.explain_dense_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True)
+        p64 = O.explain_dense_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True, dtype=torch.float64)
         assert O.rel_l2(got, port) <= max(1e-4, 3 * O.rel_l2(p64, port)), node
     printed = capsys.readouterr().out
     assert "trace is not built for inputs wider than 128 features" in printed and "Saved adjacency matrix to" in printed
@@ -369,8 +368,8 @@ def test_explainer_dropin_graph_mode(tmp_path, capsys):
         M0 = O.draw_m0(n)
         A = np.asarray(adj[g], np.float64)
         hp = O.default_hparams(num_epochs=20)
-        port = WO.explain_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True, bn=True)
-        p64 = WO.explain_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True, bn=True, dtype=torch.float64)
+        port = O.explain_dense_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True, bn=True)
+        p64 = O.explain_dense_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True, bn=True, dtype=torch.float64)
         ei, ej = np.nonzero(A)
         assert masked.shape == (n, n)
         assert O.rel_l2(masked[ei, ej], port[ei, ej]) <= max(1e-4, 3 * O.rel_l2(p64[ei, ej], port[ei, ej])), g

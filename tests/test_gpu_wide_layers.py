@@ -1,7 +1,7 @@
 """GPU (-m gpu): GCNs with hidden / output widths of 129 .. 256 on the model-variant kernel's row-block path (explain_var.cu, kBlk) and
 the model forward (forward.cu), through the C ABI, the drop-in Explainer and gnnx.dist, node and graph mode: against the masks the
-unmodified reference returned (tests/golden/wide_layers_golden.npz), against the torch port of tests/wide_oracle.py in fp32 and fp64,
-and against the narrow kernel on a zero-padded model."""
+unmodified reference returned (tests/golden/wide_layers_golden.npz), against the torch port (gnnx_oracle.explain_dense_torch) in fp32
+and fp64, and against the narrow kernel on a zero-padded model."""
 import os
 import types
 
@@ -13,7 +13,6 @@ import gnnx
 import gnnx_oracle as O
 import pool_oracle as PO
 import util
-import wide_oracle as WO
 from gnnx import _abi
 from test_gpu_deep import GG, GX_ERR_UNSUPPORTED, _args, _check, _graph_setup, _hp, _m0, _node_setup, _ohp, _state_dict, _sub, random_model
 from test_oracle_pool_ties import NEAR_TIES
@@ -94,8 +93,9 @@ def test_wide_layers_one_update_matches_fp64_port(case):
     s.eng.close()
     for t, node in enumerate(nodes):
         A, X, gt, pl, idx = _sub(s, node)
-        ref, f1 = WO.explain_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, dtype=torch.float64, return_feat=True)
-        p32, f32 = WO.explain_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, return_feat=True)
+        ref, f1 = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, dtype=torch.float64,
+                                        return_feat=True)
+        p32, f32 = O.explain_dense_torch(A, X, gt, pl, idx, s.w, dense[t], O.default_hparams(num_epochs=2), bn=bn, return_feat=True)
         assert O.rel_l2(plan.dense_of(t, out), ref) <= max(1e-5, 3 * O.rel_l2(p32, ref)), node
         assert np.abs(fm[t] - f1).max() <= max(1e-5, 3 * float(np.abs(f32 - f1).max())), node
     adj, feat, label, w, eng = _graph_setup(seed + 10, L, bn, False, hid, emb, d, 3)
@@ -110,8 +110,8 @@ def test_wide_layers_one_update_matches_fp64_port(case):
     eng.close()
     for t, g in enumerate(gids):
         args = (np.asarray(adj[g], np.float64), feat[g], int(label[g]), None, 0, w, dense[g], O.default_hparams(num_epochs=2))
-        ref, f1 = WO.explain_torch(*args, graph_mode=True, bn=bn, dtype=torch.float64, return_feat=True)
-        p32, f32 = WO.explain_torch(*args, graph_mode=True, bn=bn, return_feat=True)
+        ref, f1 = O.explain_dense_torch(*args, graph_mode=True, bn=bn, dtype=torch.float64, return_feat=True)
+        p32, f32 = O.explain_dense_torch(*args, graph_mode=True, bn=bn, return_feat=True)
         assert O.rel_l2(out[edge_off[t]:edge_off[t + 1]], ref[rc[g]]) <= max(1e-5, 3 * O.rel_l2(p32[rc[g]], ref[rc[g]])), g
         assert np.abs(fm[t] - f1).max() <= max(1e-5, 3 * float(np.abs(f32 - f1).max())), g
 
@@ -279,8 +279,8 @@ def test_explainer_dropin_node_mode(tmp_path, capsys):
         n = A.shape[0]
         M0 = O.draw_m0(n)
         hp = O.default_hparams(num_epochs=20)
-        port = WO.explain_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True)
-        p64 = WO.explain_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True, dtype=torch.float64)
+        port = O.explain_dense_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True)
+        p64 = O.explain_dense_torch(A, X, s.label[node], pl, idx, s.w, M0, hp, bn=True, dtype=torch.float64)
         assert O.rel_l2(got, port) <= max(1e-4, 3 * O.rel_l2(p64, port)), node
     printed = capsys.readouterr().out
     assert "trace is not built for --bn / num_gc_layers != 3" in printed and "Saved adjacency matrix to" in printed
@@ -307,8 +307,8 @@ def test_explainer_dropin_graph_mode(tmp_path, capsys):
         M0 = O.draw_m0(n)
         A = np.asarray(adj[g], np.float64)
         hp = O.default_hparams(num_epochs=20)
-        port = WO.explain_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True)
-        p64 = WO.explain_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True, dtype=torch.float64)
+        port = O.explain_dense_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True)
+        p64 = O.explain_dense_torch(A, feat[g], label[g], None, 0, w, M0, hp, graph_mode=True, dtype=torch.float64)
         ei, ej = np.nonzero(A)
         assert masked.shape == (n, n)
         assert O.rel_l2(masked[ei, ej], port[ei, ej]) <= max(1e-4, 3 * O.rel_l2(p64[ei, ej], port[ei, ej])), g

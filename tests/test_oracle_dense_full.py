@@ -10,7 +10,6 @@ import torch
 
 import dense_oracle as D
 import gnnx_oracle as O
-import head_oracle as HO
 import util
 
 UF = np.load(os.path.join(util.GOLDEN, "unconstrained_full_golden.npz"))
@@ -66,10 +65,10 @@ def test_port_reproduces_reference_full_mask(which, v):
     A, X, gt, y, idx, W, M0, graph, key = inputs(which, v)
     for E in (int(e) for e in UF["epochs"]):
         hp = O.default_hparams(num_epochs=E)
-        port = D.explain_dense_torch(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, full=True)
+        port = O.explain_dense_torch(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, full=True, unconstrained=True)
         ref = UF["%s_e%d_full" % (key, E)]
         assert port.shape == ref.shape and np.array_equal(port.astype(np.float32), ref), (key, E, np.abs(port - ref).max())
-        assert np.array_equal(port * A, D.explain_dense_torch(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph))
+        assert np.array_equal(port * A, O.explain_dense_torch(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, unconstrained=True))
         cf = D.explain_closed_form(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, full=True)
         for c, (r, k) in D.entry_classes(A).items():
             rec = float(UF["%s_e%d_cfdist_%s" % (key, E, c)])
@@ -94,7 +93,7 @@ def test_closed_form_full_mask_and_trace_follow_port(over):
     for graph, (A, X, gt, y, idx, M0), W in ((False, (A, X, gt, y, idx, M0), fx.weights), (True, graph_case(9), graph_weights())):
         n, d = len(A), X.shape[1]
         ptr, ctr = [], []
-        port = D.explain_dense_torch(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, trace=ptr, full=True)
+        port = O.explain_dense_torch(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, trace=ptr, full=True, unconstrained=True)
         cf = D.explain_closed_form(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, full=True, trace=ctr)
         assert len(ctr) == len(ptr) == hp.num_epochs and np.array_equal(ctr[-1]["a"], cf)
         for c, (r, k) in D.entry_classes(A).items():
@@ -119,7 +118,7 @@ def test_closed_form_head_follows_fp64_port(graph):
          "head": [(sc(24, 60), sc(24)), (sc(10, 24), sc(10))], "Wp": sc(C, 10), "bp": sc(C)}
     hp = O.default_hparams(num_epochs=6)
     cf = D.explain_closed_form(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, full=True)
-    ref = HO.explain_torch(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, dtype=torch.float64, unconstrained=True, full=True)
+    ref = O.explain_dense_torch(A, X, gt, y, idx, W, M0, hp=hp, graph_mode=graph, dtype=torch.float64, unconstrained=True, full=True)
     off = ~np.eye(len(A), dtype=bool)
     assert np.abs(cf[off] - ref[off]).max() <= 1e-9
     without = D.explain_closed_form(A, X, gt, y, idx, {k: v for k, v in W.items() if k != "head"} | {"Wp": sc(C, 60)}, M0, hp=hp,

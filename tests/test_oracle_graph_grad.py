@@ -68,7 +68,7 @@ def test_closed_form_is_autograd(golden, key):
         # the raw gradient, through the same autograd graph
         At = torch.tensor(A[None], requires_grad=True)
         xt = torch.tensor(np.asarray(X, np.float64)[None])
-        y = O._gcn_forward_torch(xt, At, GO._weights(w, torch.float64), True)
+        y = O._gcn_forward_torch(xt, At, O.weights_to_torch(w, dtype=torch.float64), True)
         (-torch.log(torch.softmax(y[0], 0)[lab])).backward()
         ref = At.grad[0].numpy()
         assert np.abs(dA - ref)[rc].max() <= 1e-10 * max(np.abs(ref[rc]).max(), 1e-30), (m, g)

@@ -16,7 +16,6 @@ import gnnx_oracle as O
 import kernel_spec as KS
 import mask_grad_oracle as MG
 import util
-import wide_oracle as WO
 from test_oracle_graph_variants import dense_m0, model_of
 from test_oracle_spec_state import _case
 
@@ -162,7 +161,8 @@ def test_specification_takes_the_ports_adam_steps(prob, hset):
     ei, ej = np.nonzero(A)
     for E in (2, 6):
         hp = O.default_hparams(num_epochs=E, **HSETS[hset])
-        port, fm = WO.explain_torch(*_args(p), p["M0"], hp=hp, graph_mode=p["graph_mode"], bn=p["bn"], dtype=torch.float64, return_feat=True)
+        port, fm = O.explain_dense_torch(*_args(p), p["M0"], hp=hp, graph_mode=p["graph_mode"], bn=p["bn"], dtype=torch.float64,
+                                         return_feat=True)
         cf = O.explain_closed_form(*_args(p), p["M0"], hp=hp, graph_mode=p["graph_mode"], bn=p["bn"])
         _, st = O.explain_closed_form(*_args(p), p["M0"], hp=O.default_hparams(num_epochs=E - 1, **HSETS[hset]), graph_mode=p["graph_mode"],
                                       bn=p["bn"], return_state=True)
@@ -182,8 +182,8 @@ def test_each_set_changes_the_result(hset):
     for prob in ("node_L3", "graph_L3"):
         p = PROBLEMS[prob]()
         ei, ej = np.nonzero(p["A"])
-        base = WO.explain_torch(*_args(p), p["M0"], hp=O.default_hparams(num_epochs=20), graph_mode=p["graph_mode"])
-        other = WO.explain_torch(*_args(p), p["M0"], hp=O.default_hparams(num_epochs=20, **HSETS[hset]), graph_mode=p["graph_mode"])
+        base = O.explain_dense_torch(*_args(p), p["M0"], hp=O.default_hparams(num_epochs=20), graph_mode=p["graph_mode"])
+        other = O.explain_dense_torch(*_args(p), p["M0"], hp=O.default_hparams(num_epochs=20, **HSETS[hset]), graph_mode=p["graph_mode"])
         assert O.rel_l2(other[ei, ej], base[ei, ej]) > 1e-2, (prob, hset)
 
 

@@ -4,8 +4,9 @@ tests/test_gpu_mask_grads.py can compare the kernels' gradients with it:
   * the default model and its depth / --bn variants, node and graph mode: the gM / gF gnnx_oracle.explain_closed_form reports after one
     update from that state (init_state), to 1e-9; inputs wider than 128 (the wide path's d) the same way;
   * attention models: att_oracle.mask_grads_closed_form;
-  * every other model (5 / 7 layers, widths to 256, MLP heads, unconstrained=True): one fp64 SGD step of the torch ports (wide_oracle,
-    head_oracle) from a symmetric M0 lands on M0 - lr g, and dense_oracle.explain_closed_form's gradient for unconstrained=True."""
+  * every other model (5 / 7 layers, widths to 256, MLP heads, unconstrained=True): one fp64 SGD step of the torch port
+    (gnnx_oracle.explain_dense_torch) from a symmetric M0 lands on M0 - lr g, and dense_oracle.explain_closed_form's gradient for
+    unconstrained=True."""
 import numpy as np
 import pytest
 import torch
@@ -13,9 +14,7 @@ import torch
 import att_oracle as AO
 import dense_oracle as D
 import gnnx_oracle as O
-import head_oracle as HO
 import mask_grad_oracle as MG
-import wide_oracle as WO
 from test_oracle_att import random_att_model, random_graph
 from test_oracle_hparams import PROBLEMS, _args
 
@@ -88,7 +87,7 @@ def test_attention_equals_its_closed_form(L, bn, graph_mode):
     M, F = _point(rng, 12, 7)
     pl = rng.integers(0, 4, 12)
     gM, gF = AO.mask_grads_closed_form(A, X, 1, pl, 2, w, M, F, graph_mode=graph_mode, bn=bn)
-    g = MG.mask_grads(A, X, 1, pl, 2, w, M, F, HP, graph_mode=graph_mode, bn=bn, att=True)
+    g = MG.mask_grads(A, X, 1, pl, 2, w, M, F, HP, graph_mode=graph_mode, bn=bn)
     assert _close(g.gM, gM) and _close(g.gF, gF)
 
 
@@ -114,12 +113,11 @@ def test_other_models_take_the_ports_sgd_step(case, graph_mode):
     n, d, hid, emb, C, L, head, bn = OTHER[case]
     rng, w, A, X, pl = _random_problem(100 + list(OTHER).index(case), n, d, hid, emb, C, L, head, bn)
     M0, _ = _point(rng, n, d, sym=True)
-    g = MG.mask_grads(A, X, 1, None if graph_mode else pl, 2, w, M0, np.zeros(d), HP, graph_mode=graph_mode, bn=bn, head=bool(head))
+    g = MG.mask_grads(A, X, 1, None if graph_mode else pl, 2, w, M0, np.zeros(d), HP, graph_mode=graph_mode, bn=bn)
     ei, ej = np.nonzero(A)
     lr = 1e-3 / np.abs(g.gM).max()
-    port = (lambda **kw: HO.explain_torch(**kw)) if head else (lambda **kw: WO.explain_torch(**kw))
-    gM, gF = _sgd_step_grads(port, A, M0, lr, sub_adj=A, sub_feat=X, gt_label=1, pred_label=None if graph_mode else pl, node_idx_new=2,
-                             weights=w, graph_mode=graph_mode, bn=bn)
+    gM, gF = _sgd_step_grads(O.explain_dense_torch, A, M0, lr, sub_adj=A, sub_feat=X, gt_label=1, pred_label=None if graph_mode else pl,
+                             node_idx_new=2, weights=w, graph_mode=graph_mode, bn=bn)
     assert np.abs(gM - g.gM[ei, ej]).max() <= 1e-7 * np.abs(g.gM).max(), case
     assert np.abs(gF - g.gF).max() <= 1e-7 * np.abs(g.gF).max(), case
 
@@ -128,17 +126,17 @@ def test_other_models_take_the_ports_sgd_step(case, graph_mode):
 @pytest.mark.parametrize("model", ["default", "bn", "head"])
 def test_unconstrained_mask(model, graph_mode):
     """unconstrained=True: every entry of the dense mask against dense_oracle's closed form (plain models) or, with a head, the edges of
-    head_oracle's unconstrained port after one SGD step."""
+    the unconstrained port after one SGD step."""
     rng, w, A, X, pl = _random_problem(7 + len(model), 15, 8, 20, 20, 3, 3, [50] if model == "head" else None)
     bn = model == "bn"
     M0, _ = _point(rng, 15, 8, sym=True)
-    kw = dict(graph_mode=graph_mode, bn=bn, head=model == "head", unconstrained=True)
+    kw = dict(graph_mode=graph_mode, bn=bn, unconstrained=True)
     g = MG.mask_grads(A, X, 1, None if graph_mode else pl, 2, w, M0, np.zeros(8), HP, **kw)
     assert np.abs(g.gF - 0.25 * HP.feat_size / 8).max() <= 1e-15          # the forward never sees F
     if model == "head":
         lr = 1e-3 / np.abs(g.gM).max()
         ei, ej = np.nonzero(A)
-        gM, _ = _sgd_step_grads(lambda **k: HO.explain_torch(**k), A, M0, lr, sub_adj=A, sub_feat=X, gt_label=1,
+        gM, _ = _sgd_step_grads(O.explain_dense_torch, A, M0, lr, sub_adj=A, sub_feat=X, gt_label=1,
                                 pred_label=None if graph_mode else pl, node_idx_new=2, weights=w, graph_mode=graph_mode, bn=bn,
                                 unconstrained=True)
         assert np.abs(gM - g.gM[ei, ej]).max() <= 1e-7 * np.abs(g.gM).max()

@@ -1,5 +1,5 @@
-"""CPU: graph mode's max-pool arg-max routing in the torch ports (tests/pool_oracle.py).  The ports with the readout made visible are
-bit for bit the ports; the one graph of the fixtures a kernel cannot be held to 1e-4 of the reference on (graphs_h256, graph 8) is a
+"""CPU: graph mode's max-pool arg-max routing in the torch port (tests/pool_oracle.py).  The port with the readout made visible is
+bit for bit the port; the one graph of the fixtures a kernel cannot be held to 1e-4 of the reference on (graphs_h256, graph 8) is a
 sub-ulp arg-max margin whose flip moves the final mask by 3.66e-4; exact ties route to the first maximal row, like torch.max."""
 import importlib
 import os
@@ -10,7 +10,6 @@ import torch
 
 import gnnx_oracle as O
 import pool_oracle as P
-import wide_oracle as WO
 from test_oracle_deep import golden_items
 from test_oracle_wide_layers import GOLDEN, case_weights
 
@@ -56,7 +55,7 @@ def _h256(gi):
 def test_unflipped_port_is_bit_identical():
     g, key, A, X, gt, w, M0, hp, bn = _h256(8)
     for dtype in (torch.float, torch.float64):
-        ref, fref = WO.explain_torch(A, X, gt, None, 0, w, M0, hp, graph_mode=True, bn=bn, dtype=dtype, return_feat=True)
+        ref, fref = O.explain_dense_torch(A, X, gt, None, 0, w, M0, hp, graph_mode=True, bn=bn, dtype=dtype, return_feat=True)
         got, fgot, rec = P.explain_torch_pool(A, X, gt, w, M0, hp, bn=bn, dtype=dtype, record=True)
         assert np.array_equal(got, ref) and np.array_equal(fgot, fref)
         assert len(rec) == hp.num_epochs - 1

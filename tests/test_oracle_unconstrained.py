@@ -9,6 +9,7 @@ import torch
 
 import dense_oracle as D
 import gnnx_oracle as O
+import mask_grad_oracle as MG
 import util
 
 U = np.load(os.path.join(util.GOLDEN, "unconstrained_golden.npz"))
@@ -43,7 +44,7 @@ def test_port_reproduces_reference_nodes(which, nodes, epochs):
     for node in nodes or [int(v) for v in U[which + "_nodes"]]:
         A, X, gt, y, idx, M0, (ei, ej) = node_case(fx, node)
         for E in epochs:
-            out = D.explain_dense_torch(A, X, gt, y, idx, fx.weights, M0, hp=O.default_hparams(num_epochs=E))
+            out = O.explain_dense_torch(A, X, gt, y, idx, fx.weights, M0, hp=O.default_hparams(num_epochs=E), unconstrained=True)
             assert O.rel_l2(out[ei, ej], U["%s_n%d_e%d_mask" % (which, node, E)]) == 0.0, (which, node, E)
 
 
@@ -52,7 +53,7 @@ def test_port_reproduces_reference_graphs(epochs):
     W = graph_weights()
     for g in range(int(GG["num_graphs"])):
         A, X, gt, _, _, M0, (ei, ej) = graph_case(g)
-        out = D.explain_dense_torch(A, X, gt, None, 0, W, M0, hp=O.default_hparams(num_epochs=epochs), graph_mode=True)
+        out = O.explain_dense_torch(A, X, gt, None, 0, W, M0, hp=O.default_hparams(num_epochs=epochs), graph_mode=True, unconstrained=True)
         assert O.rel_l2(out[ei, ej], U["graphs_g%d_e%d_mask" % (g, epochs)]) == 0.0, (g, epochs)
 
 
@@ -68,12 +69,14 @@ def test_port_reproduces_reference_variants(tag):
         A = O.dense_from_csr(srp, scol); ei, ej = np.nonzero(A)
         pred_label = fx.pred_label if tag == "sgd" else variant_pred_label(fx, Wn, L, bn)
         M0 = O.draw_m0(len(nbrs), seed=int(fx.gold["n%d_seed" % node]))
-        out = D.explain_dense_torch(A, X, int(lab[idx]), pred_label[nbrs], idx, Wn, M0, hp=O.default_hparams(num_epochs=E, **over), bn=bn)
+        out = O.explain_dense_torch(A, X, int(lab[idx]), pred_label[nbrs], idx, Wn, M0, hp=O.default_hparams(num_epochs=E, **over), bn=bn,
+                                    unconstrained=True)
         assert O.rel_l2(out[ei, ej], U["var_%s_rand_n%d_mask" % (tag, node)]) == 0.0, (tag, node)
     Wg = graph_weights() if tag == "sgd" else var_weights(tag, "graphs")
     for g in (0, 5, 11):
         A, X, gt, _, _, M0, (ei, ej) = graph_case(g)
-        out = D.explain_dense_torch(A, X, gt, None, 0, Wg, M0, hp=O.default_hparams(num_epochs=E, **over), graph_mode=True, bn=bn)
+        out = O.explain_dense_torch(A, X, gt, None, 0, Wg, M0, hp=O.default_hparams(num_epochs=E, **over), graph_mode=True, bn=bn,
+                                    unconstrained=True)
         assert O.rel_l2(out[ei, ej], U["var_%s_graphs_g%d_mask" % (tag, g)]) == 0.0, (tag, g)
 
 
@@ -94,33 +97,11 @@ def test_port_prints_reference_rows(which):
     for node in [int(v) for v in U["trace_%s_nodes" % which]]:
         A, X, gt, y, idx, M0, _ = node_case(fx, node)
         tr = []
-        D.explain_dense_torch(A, X, gt, y, idx, fx.weights, M0, hp=O.default_hparams(num_epochs=E), trace=tr)
+        O.explain_dense_torch(A, X, gt, y, idx, fx.weights, M0, hp=O.default_hparams(num_epochs=E), trace=tr, unconstrained=True)
         ref = U["trace_%s_n%d" % (which, node)]
         got = np.array([[t["loss"], t["density"]] + list(t["pred"]) for t in tr])
         # the reference prints 8 decimals of every value: the port must agree to that print precision
         assert np.abs(got - ref).max() <= 5e-8 + 1e-7 * np.abs(ref).max(), (which, node, np.abs(got - ref).max())
-
-
-def _autograd_grads(A, X, gt, y, idx, W, M0, graph_mode, bn):
-    """fp64 torch autograd of the unconstrained loss (explain.py:688-692,740-808) at M0, F = 0: (dL/dM, dL/dF)."""
-    hp = O.default_hparams()
-    t = lambda v: torch.tensor(np.asarray(v), dtype=torch.float64)
-    Wt = dict(conv_w=[t(W["W%d" % l]) for l in range(1, 5) if "W%d" % l in W],
-              conv_b=[t(W["b%d" % l]) for l in range(1, 5) if "W%d" % l in W], pred_w=t(W["Wp"]), pred_b=t(W["bp"]))
-    n, d = X.shape
-    M = t(M0).requires_grad_(True)
-    F = torch.zeros(d, dtype=torch.float64, requires_grad=True)
-    S = torch.sigmoid(M)
-    a = ((S + S.t()) / 2 * (1 - torch.eye(n, dtype=torch.float64)))[None]
-    logits = O._gcn_forward_torch(t(X)[None], a, Wt, graph_mode, bn)
-    p = torch.softmax(logits[0] if graph_mode else logits[0, idx], 0)
-    loss = -torch.log(p[gt]) + hp.size * S.sum() + hp.feat_size * torch.sigmoid(F).mean()
-    loss = loss + hp.ent * (-S * torch.log(S) - (1 - S) * torch.log(1 - S)).mean()
-    if not graph_mode:
-        yt = t(y)
-        loss = loss + hp.lap * (yt @ (torch.diag(a[0].sum(0)) - a[0]) @ yt) / (n * n)
-    loss.backward()
-    return M.grad.numpy(), F.grad.numpy()
 
 
 @pytest.mark.parametrize("case", ["node", "node_bn", "node_L4", "graph", "graph_bn", "graph_L4"])
@@ -138,7 +119,8 @@ def test_closed_form_gradient_matches_autograd(case):
         A, X, gt, y, idx, M0, _ = node_case(fx, 33, n_hops=4 if tag == "L4" else 3)
     _, st = D.explain_closed_form(A, X, gt, y, idx, W, M0, hp=O.default_hparams(num_epochs=1), graph_mode=graph_mode, bn=bn,
                                   return_state=True)
-    gM, gF = _autograd_grads(A, X, gt, y, idx, W, M0, graph_mode, bn)
+    g = MG.mask_grads(A, X, gt, y, idx, W, M0, np.zeros(X.shape[1]), O.default_hparams(), graph_mode=graph_mode, bn=bn, unconstrained=True)
+    gM, gF = g.gM, g.gF
     assert np.abs(gM).max() > 0 and np.abs(gF).max() > 0
     assert np.abs(st["gM"] - gM).max() <= 1e-9 * max(1.0, np.abs(gM).max()), case
     assert np.abs(st["gF"] - gF).max() <= 1e-9, case
@@ -154,12 +136,12 @@ def test_closed_form_follows_port(opt):
     fx = util.load_fixture("rand")
     for node in (33, 149):
         A, X, gt, y, idx, M0, (ei, ej) = node_case(fx, node)
-        port = D.explain_dense_torch(A, X, gt, y, idx, fx.weights, M0, hp=hp)
+        port = O.explain_dense_torch(A, X, gt, y, idx, fx.weights, M0, hp=hp, unconstrained=True)
         cf = D.explain_closed_form(A, X, gt, y, idx, fx.weights, M0, hp=hp)
         assert O.rel_l2(cf[ei, ej], port[ei, ej]) <= 1e-6, (opt, node, O.rel_l2(cf[ei, ej], port[ei, ej]))
     W = graph_weights()
     for g in (2, 9):
         A, X, gt, _, _, M0, (ei, ej) = graph_case(g)
-        port = D.explain_dense_torch(A, X, gt, None, 0, W, M0, hp=hp, graph_mode=True)
+        port = O.explain_dense_torch(A, X, gt, None, 0, W, M0, hp=hp, graph_mode=True, unconstrained=True)
         cf = D.explain_closed_form(A, X, gt, None, 0, W, M0, hp=hp, graph_mode=True)
         assert O.rel_l2(cf[ei, ej], port[ei, ej]) <= 1e-6, (opt, g, O.rel_l2(cf[ei, ej], port[ei, ej]))

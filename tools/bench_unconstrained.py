@@ -5,8 +5,8 @@
 Workloads: syn1, all 700 nodes x 100 epochs (node mode, the fixture's model), and bench.py's configs[3] stand-in (4337 padded
 molecule-like graphs, max_nodes 100, d = 14, 100 epochs; graph mode).  Philox init.  Prints one JSON line: per workload the device
 time of gx_explain_{nodes,graphs}_unconstrained (CUDA events after warm-up, L2 flushed between steps, plan outside) as items/s,
-the GPU's name and power limit, and the line-by-line CPU port's rate (tests/dense_oracle.explain_dense_torch) on S evenly spaced
-items.  Also the time of ONE task near the size limit (a 3-hop subgraph of n = 3769 in a Barabasi-Albert graph, 100 epochs): one CTA
+the GPU's name and power limit, and the line-by-line CPU port's rate (gnnx_oracle.explain_dense_torch, unconstrained=True) on S evenly
+spaced items.  Also the time of ONE task near the size limit (a 3-hop subgraph of n = 3769 in a Barabasi-Albert graph, 100 epochs): one CTA
 per task, so this is the latency of the largest task a batch can hold.  Writes nothing.
 """
 import argparse
@@ -56,7 +56,6 @@ def main():
     a = ap.parse_args()
     a.gpus = 1
     import gnnx
-    import dense_oracle as D
     import gnnx_oracle as O
     from gnnx import _abi
     c = gpu_ctx(a)
@@ -78,8 +77,9 @@ def main():
     def node_item(v):
         idx, srp, scol, X, lab, nbrs = O.extract_neighborhood(g["rowptr"], g["col"], g["feat"], g["label"], int(v), 3)
         A = O.dense_from_csr(srp, scol)
-        return lambda: D.explain_dense_torch(A, X, int(lab[idx]), g["pred_label"][nbrs], idx, g["weights"], O.draw_m0(len(nbrs), seed=int(v)),
-                                             hp=O.default_hparams(num_epochs=NUM_EPOCHS))
+        return lambda: O.explain_dense_torch(A, X, int(lab[idx]), g["pred_label"][nbrs], idx, g["weights"],
+                                             O.draw_m0(len(nbrs), seed=int(v)),
+                                             hp=O.default_hparams(num_epochs=NUM_EPOCHS), unconstrained=True)
     sample = nodes[np.linspace(0, len(nodes) - 1, a.cpu_sample).astype(int)]
     r.update(unit="nodes/s", workload="syn1, all %d nodes x %d epochs, 3 hops" % (len(nodes), NUM_EPOCHS),
              n_mean=float(n_t.mean()), n_max=int(n_t.max()),
@@ -103,8 +103,8 @@ def main():
     gsample = np.linspace(0, G - 1, a.cpu_sample).astype(int)
 
     def graph_item(k):
-        return lambda: D.explain_dense_torch(adj[k].astype(np.float64), feat[k], int(label[k]), None, 0, W, O.draw_m0(n, seed=k),
-                                             hp=O.default_hparams(num_epochs=NUM_EPOCHS), graph_mode=True)
+        return lambda: O.explain_dense_torch(adj[k].astype(np.float64), feat[k], int(label[k]), None, 0, W, O.draw_m0(n, seed=k),
+                                             hp=O.default_hparams(num_epochs=NUM_EPOCHS), graph_mode=True, unconstrained=True)
     r.update(unit="graphs/s", workload="configs[3] stand-in: %d padded graphs (max_nodes %d, d=%d) x %d epochs, random 3-layer model" % (G, n, d, NUM_EPOCHS),
              cpu_port_graphs_per_s=_cpu_rate([graph_item(int(k)) for k in gsample]), cpu_port_sample=[int(k) for k in gsample])
     res["graphs"] = r

@@ -7,7 +7,7 @@ of width d = 256 and d = 1433, all 700 nodes (node mode, 3 hops), and the 12-gra
 one-hot features over 190 labels (graph mode).  Prints one JSON line: per workload the device time of one gx_explain_nodes /
 gx_explain_graphs call (CUDA events after warm-up, L2 flushed between steps, plan outside) as items/s over WINDOWS windows of at least
 one second each (median, and the min / max as the spread), the SM clock sampled during the first window, the CPU port's rate on a few
-items of the same workload (tests/wide_oracle.py, fp32 torch, one process), and the GPU's name and power limit.  Writes nothing.
+items of the same workload (gnnx_oracle.explain_dense_torch, fp32 torch, one process), and the GPU's name and power limit.  Writes nothing.
 """
 import argparse
 import ctypes as C
@@ -84,7 +84,6 @@ def main():
     a.gpus = 1
     import gnnx
     import gnnx_oracle as O
-    import wide_oracle as WO
     from gnnx import _abi
     c = gpu_ctx(a)
     name, power = _gpu_name_power(c.local_rank)
@@ -111,7 +110,7 @@ def main():
             A = O.dense_from_csr(srp, scol)
             M0 = O.draw_m0(len(nbrs), seed=node)
             items.append(lambda A=A, sfeat=sfeat, gt=slabel[idx], pl=g["pred_label"][nbrs], idx=idx, M0=M0:
-                         WO.explain_torch(A, sfeat, gt, pl, idx, w, M0, hp))
+                         O.explain_dense_torch(A, sfeat, gt, pl, idx, w, M0, hp))
         r["cpu_port"] = {"value": _port_rate(items), "unit": "nodes/s", "items": len(items)} if items else None
         res["syn1_d%d_nodes" % d] = r
     gg = np.load(os.path.join(ROOT, "tests", "golden", "graphs_golden.npz"))
@@ -129,7 +128,7 @@ def main():
     r = _device_rate(c, eng, lib.gx_explain_graphs, G, te, a)
     eng.close()
     r.update(unit="graphs/s", workload="12-graph stand-in (max_nodes %d), one-hot features d=%d, x %d epochs" % (adj.shape[1], d, NUM_EPOCHS))
-    items = [lambda gi=gi: WO.explain_torch(np.asarray(adj[gi], np.float64), feat[gi], int(label[gi]), None, 0, w,
+    items = [lambda gi=gi: O.explain_dense_torch(np.asarray(adj[gi], np.float64), feat[gi], int(label[gi]), None, 0, w,
                                             O.draw_m0(adj.shape[1], seed=gi), hp, graph_mode=True) for gi in range(min(a.port_items, G))]
     r["cpu_port"] = {"value": _port_rate(items), "unit": "graphs/s", "items": len(items)} if items else None
     res["graphs_d190"] = r

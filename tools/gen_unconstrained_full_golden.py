@@ -15,7 +15,7 @@ Keys (full masks float32 (n, n), row-major as the reference's; spreads float64):
 The spread of a class is the reproducibility of the reference itself, as oracle/gen_sensitivity.py measures it: the largest rel-L2,
 over the class's entries, of the line-by-line port from the reference's mask when every M0 entry is nudged by +-1 ulp (twelve random
 sign patterns; four more that also nudge every model weight).  cfdist is the rel-L2 of the fp64 closed form from the port.  The port
-(tests/dense_oracle.py) must reproduce every full reference mask bit for bit.
+(oracle/gnnx_oracle.explain_dense_torch, unconstrained=True) must reproduce every full reference mask bit for bit.
 """
 import os
 import sys
@@ -111,7 +111,7 @@ def gen(R):
                 M0 = O.draw_m0(len(nbrs), seed=seed)
                 key = "%s_n%d_e%d" % (fx, node, E)
                 sp = _record(out, key, A, full,
-                             lambda M, Wx: D.explain_dense_torch(A, sub_feat, gt, pl, idx, Wx, M, hp=hp, full=True),
+                             lambda M, Wx: O.explain_dense_torch(A, sub_feat, gt, pl, idx, Wx, M, hp=hp, full=True, unconstrained=True),
                              lambda M: D.explain_closed_form(A, sub_feat, gt, pl, idx, W, M, hp=hp, full=True), M0, W, node)
                 out["%s_n%d_nbrs" % (fx, node)] = np.asarray(nbrs, np.int32)
                 print("  %s n=%d: %s" % (key, len(nbrs), {c: "%.1e" % v for c, v in sp.items()}), flush=True)
@@ -145,7 +145,8 @@ def gen(R):
             M0 = O.draw_m0(n, seed=seed)
             key = "graphs_g%d_e%d" % (g, E)
             sp = _record(out, key, adj[g], full,
-                         lambda M, Wx: D.explain_dense_torch(adj[g], feat[g], int(label[g]), None, 0, Wx, M, hp=hp, graph_mode=True, full=True),
+                         lambda M, Wx: O.explain_dense_torch(adj[g], feat[g], int(label[g]), None, 0, Wx, M, hp=hp, graph_mode=True,
+                                                             full=True, unconstrained=True),
                          lambda M: D.explain_closed_form(adj[g], feat[g], int(label[g]), None, 0, W, M, hp=hp, graph_mode=True, full=True),
                          M0, W, 100 + g)
             print("  %s: %s" % (key, {c: "%.1e" % v for c, v in sp.items()}), flush=True)

@@ -15,7 +15,8 @@ Keys (masks at the sub-adjacency entries, row-major, float32; spreads float64):
 The spread of a case is the reproducibility of the reference itself: how far the line-by-line port moves from the reference's mask
 when every M0 entry is nudged by +-1 ulp (nudges draws), and how far the fp64 and fp32 closed forms (the same trajectory restated in
 another summation order) land from it.  Some dense trajectories are insensitive to M0 noise but not to the order of the sums (a
-graph whose fp32 closed form lands 0.14 away at 100 epochs), hence both.  The port (tests/dense_oracle.py) must reproduce every reference mask to below 1e-6.
+graph whose fp32 closed form lands 0.14 away at 100 epochs), hence both.  The port (gnnx_oracle.explain_dense_torch,
+unconstrained=True) must reproduce every reference mask to below 1e-6.
 """
 import contextlib
 import io
@@ -98,7 +99,7 @@ def _explain_nodes(R, O, out, key, ex, nodes, seeds, W, hp_over, epochs, bn, nud
         pl = np.argmax(np.asarray(ex.pred[0])[nbrs], axis=1)
         gt = int(np.asarray(sub_label)[idx])
         A = np.asarray(sub_adj, np.float64)
-        port = lambda M: D.explain_dense_torch(A, sub_feat, gt, pl, idx, W, M, hp=hp, bn=bn)
+        port = lambda M: O.explain_dense_torch(A, sub_feat, gt, pl, idx, W, M, hp=hp, bn=bn, unconstrained=True)
         cf = lambda M, dt: D.explain_closed_form(A, sub_feat, gt, pl, idx, W, M, hp=hp, bn=bn, dtype=dt)
         out[key % node + "_mask"] = ref.astype(np.float32)
         out[key % node + "_spread"] = np.float64(_check(O, port, cf, M0, ref, ei, ej, nudges, node, (key % node)))
@@ -128,7 +129,8 @@ def _explain_graphs(R, O, out, key, model, gg, W, L, bn, hp_over, epochs, nudges
         off = masked.copy(); off[ei, ej] = 0
         assert np.all(off == 0)
         ref = masked[ei, ej]
-        port = lambda M: D.explain_dense_torch(adj[g], feat[g], int(label[g]), None, 0, W, M, hp=hp, graph_mode=True, bn=bn)
+        port = lambda M: O.explain_dense_torch(adj[g], feat[g], int(label[g]), None, 0, W, M, hp=hp, graph_mode=True, bn=bn,
+                                               unconstrained=True)
         cf = lambda M, dt: D.explain_closed_form(adj[g], feat[g], int(label[g]), None, 0, W, M, hp=hp, graph_mode=True, bn=bn, dtype=dt)
         out[key % g + "_mask"] = ref.astype(np.float32)
         out[key % g + "_spread"] = np.float64(_check(O, port, cf, M0, ref, ei, ej, nudges, 100 + g, key % g))

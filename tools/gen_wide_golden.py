@@ -17,8 +17,8 @@ Keys (masks at the sub-adjacency entries, row-major, float32; spreads float64):
   <case>_nodes, <case>_n<node>_seed / _nbrs / _mask / _spread   node mode
   <case>_g<g>_mask / _spread                       graph mode (M0 seeds: graphs_golden.npz g<g>_seed)
 The spread of a mask is the reproducibility of the reference itself: the largest distance from the reference's mask of the torch port
-(tests/wide_oracle.py) run with every M0 entry nudged by +-1 ulp (NUDGES draws), and of the same port in fp64.  The port must land
-within max(1e-6, 3 x spread) of every reference mask.
+(gnnx_oracle.explain_dense_torch) run with every M0 entry nudged by +-1 ulp (NUDGES draws), and of the same port in fp64.  The port
+must land within max(1e-6, 3 x spread) of every reference mask.
 """
 import os
 import sys
@@ -31,7 +31,6 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import gnnx_oracle as O  # noqa: E402
 import ref_harness  # noqa: E402
-import wide_oracle as WO  # noqa: E402
 from gen_golden import OUT, train_args  # noqa: E402
 
 NUDGES = 3
@@ -112,7 +111,7 @@ def gen_node_case(R, out, name, L, bn, opt, epochs, seed):
         pl = np.argmax(pred[0].numpy()[nbrs], axis=1)
         gt = int(np.asarray(sub_label)[idx])
         A = np.asarray(sub_adj, np.float64)
-        port = lambda M, dt: WO.explain_torch(A, np.asarray(sub_feat, np.float32), gt, pl, idx, W, M, hp, bn=bn, dtype=dt)
+        port = lambda M, dt: O.explain_dense_torch(A, np.asarray(sub_feat, np.float32), gt, pl, idx, W, M, hp, bn=bn, dtype=dt)
         key = "%s_n%d" % (name, node)
         out[key + "_seed"] = np.int64(seed_n)
         out[key + "_nbrs"] = np.asarray(nbrs, np.int32)
@@ -147,7 +146,7 @@ def gen_graph_case(R, out, name, L, bn, opt, epochs, seed):
             masked = np.asarray(ex.explain(node_idx=0, graph_idx=g, graph_mode=True))
         ei, ej = np.nonzero(adj[g])
         ref = masked[ei, ej]
-        port = lambda M, dt: WO.explain_torch(adj[g], feat[g], int(label[g]), None, 0, W, M, hp, graph_mode=True, bn=bn, dtype=dt)
+        port = lambda M, dt: O.explain_dense_torch(adj[g], feat[g], int(label[g]), None, 0, W, M, hp, graph_mode=True, bn=bn, dtype=dt)
         out["%s_g%d_mask" % (name, g)] = ref.astype(np.float32)
         out["%s_g%d_spread" % (name, g)] = np.float64(_spread(port, M0, ref, ei, ej, 100 + g, "%s_g%d" % (name, g)))
     print("  %s: spreads %s" % (name, ["%.1e" % out["%s_g%d_spread" % (name, g)] for g in range(G_n)]), flush=True)
